@@ -11,6 +11,10 @@ The default line also carries the single-chunk measurement of the same process u
 Weak scaling: per-GPU work is fixed.
 Decode length is pinned (SURVEY.md §8d): prompt of 4 tokens, exactly 128 new tokens (EOT in suppress_tokens).
 
+``--dump-outputs DIR`` writes what the timed engine path returned in its last step (token ids, scores, no-speech
+probabilities, a fixed seeded sample of the encoder output) as ``DIR/<name>.npy``; the inputs depend only on the
+arguments, so two builds can be compared output for output.
+
 Prints ONE JSON line (rank 0).  ``value`` = audio seconds per second through the engine calls (encode_audio + generate; the
 1.92 MB/chunk PCM upload is inside, see ``stages_ms.h2d``), timed with CUDA events on the engine's stream around the K steps
 (barrier + sync on both sides, max over ranks; the host wall clock of the same region is in ``host_wall_ms_per_step``);
@@ -44,11 +48,12 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16 (a 700 W card; a lower power limit lowers the reachable rate)
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -250,7 +255,7 @@ def run_engine(args):
         if use_dist:
             dist.barrier()
 
-    def measure(workload: str, steps: int, warmup: int, sample_clocks: bool):
+    def measure(workload: str, steps: int, warmup: int, sample_clocks: bool, dump_dir=None):
         """One workload: W warm-up steps, K steps through the engine calls, K steps through the public API."""
         B = 1 if workload == "single" else args.batch_size
         chunks = [synthetic_audio(rank * 1000 + i, 30.0) for i in range(B)]
@@ -258,11 +263,14 @@ def run_engine(args):
         clips = [{"start": 30.0 * i, "end": 30.0 * (i + 1)} for i in range(B)]
         walls = []
 
+        last = {}
+
         def engine_step():
             enc = eng.encode_audio(chunks)
             res = eng.generate(enc, [prompt] * B, beam_size=args.beam_size, max_length=len(prompt) + NEW_TOKENS, suppress_tokens=suppress,
                                return_scores=True, return_no_speech_prob=True)
             assert all(len(r.sequences_ids[0]) == NEW_TOKENS for r in res)
+            last["enc"], last["res"] = enc, res
             return res
 
         def api_step():
@@ -302,6 +310,8 @@ def run_engine(args):
         dt = timed(engine_step)
         stats = eng.timing()
         eng.timing(enable=False)
+        if dump_dir and rank == 0:
+            dump_outputs(dump_dir, workload, last["enc"], last["res"])
         dt_api = timed(api_step)
         clocks = sampler.stop() if sampler else None
 
@@ -313,7 +323,6 @@ def run_engine(args):
         enc_flops = enc_flops_per_chunk(dims) * B * steps
         enc_tf = enc_flops / (stats["encoder_ms"] * 1e-3) / 1e12 if stats["encoder_ms"] > 0 else 0.0
         kernel = "dstep_kernel" if R <= 8 else "bstep_kernel"
-        traffic, traffic_note = ncu_traffic(kernel)
         return dict(
             B=B, value=audio_s / dt, e2e_value=audio_s / dt_api, ms_per_step=dt / steps * 1e3, e2e_ms_per_step=dt_api / steps * 1e3,
             rtf=dt / audio_s * world, h2d=int(audio.nbytes), d2h=int(B * (448 * 4 + 16)), launches=int(stats["launches"]), clocks=clocks,
@@ -323,12 +332,12 @@ def run_engine(args):
             roofline={"bound": "hbm",
                       "kernel": f"decode step = {kernel} (persistent cooperative kernel: weight stream + self/cross attention + logits) + 2 search kernels",
                       "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "peak_source": pk["source"],
-                      "traffic": traffic, "traffic_source": traffic_note, "ms_per_decode_step": dec_ms / steps_dec,
+                      "ms_per_decode_step": dec_ms / steps_dec,
                       "alg_bytes_per_step": stats["decode_alg_bytes"] / steps_dec},
             roofline_encoder={"bound": "tensor", "achieved": enc_tf, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": enc_tf / pk["tflops"],
                               "flops_per_chunk": enc_flops_per_chunk(dims), "ms_per_chunk": stats["encoder_ms"] / (B * steps)})
 
-    m = measure(args.workload, args.steps, args.warmup, True)
+    m = measure(args.workload, args.steps, args.warmup, True, args.dump_outputs)
     B = m["B"]
     line = dict(
         metric=METRIC, value=m["value"], unit="audio-s/s", n_gpus=world, steps=args.steps, warmup=max(args.warmup, 3),
@@ -336,7 +345,7 @@ def run_engine(args):
         dtype="int8" if args.compute_type.startswith("int8") else "f16", data="synthetic", rtf=m["rtf"],
         config={"workload": workload_name(args), "model": args.model, "global_batch": B * world, "beam_size": args.beam_size,
                 "new_tokens": NEW_TOKENS, "parallelism": f"chunk-parallel replicas x{world}", "compute_type": args.compute_type,
-                "l2": "working set per step (3.1 GB weights + 0.25 GB/chunk cross-KV) exceeds the 126 MB L2; no flush needed",
+                "l2": "working set per step (3.1 GB weights + 0.25 GB/chunk cross-KV) exceeds the 50 MB L2; no flush needed",
                 "weights": f"synthetic seed {args.seed}, exact {args.model} shapes", "load_s": round(t_load, 1)},
         e2e={"value": m["e2e_value"], "unit": "audio-s/s", "h2d_bytes_per_step": m["h2d"], "d2h_bytes_per_step": m["d2h"],
              "api": "BatchedInferencePipeline.transcribe(ndarray, clip_timestamps=..., batch_size=%d)" % B, "ms_per_step": m["e2e_ms_per_step"]},
@@ -362,30 +371,16 @@ def run_engine(args):
         print(json.dumps(line), flush=True)
 
 
-def ncu_traffic(kernel: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, from the committed `ncu --set full` capture
-    (profiles/r2_ncu_traffic.json).  The file records a fingerprint of the kernel's source code at capture time: when the code has
-    changed since, the number is stale and is NOT reported (traffic = null, and a loud note on stderr)."""
-    import hashlib
-
-    p = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    try:
-        with open(p) as f:
-            d = json.load(f)
-        ent = d.get(kernel)
-        if not ent:
-            return None, "no capture committed for " + kernel
-        src = os.path.join(ROOT, "faster_whisper_b200", "csrc", ent["source_file"])
-        from faster_whisper_b200.build import source_fingerprint
-
-        sha = source_fingerprint(src)  # code only: blank lines and whole-line comments do not count
-        if sha != ent.get("source_sha16"):
-            sys.stderr.write(f"[bench] profiles/r2_ncu_traffic.json is STALE for {kernel}: {ent['source_file']} changed since the ncu capture "
-                             f"({ent.get('source_sha16')} -> {sha}); roofline.traffic is reported as null\n")
-            return None, "stale: source changed since the capture"
-        return ent["dram_bytes_per_launch"], ent.get("capture", "profiles/")
-    except (OSError, ValueError, KeyError) as e:
-        return None, f"unavailable: {e}"
+def dump_outputs(d: str, workload: str, enc, res) -> None:
+    """The arrays a caller of the timed path receives from its last step, as float32 / float64 .npy files (under 64 MB in all)."""
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, f"{workload}_tokens.npy"), np.asarray([r.sequences_ids[0] for r in res], dtype=np.float64))
+    np.save(os.path.join(d, f"{workload}_scores.npy"), np.asarray([r.scores[0] for r in res], dtype=np.float64))
+    np.save(os.path.join(d, f"{workload}_no_speech_prob.npy"), np.asarray([r.no_speech_prob for r in res], dtype=np.float64))
+    e = np.asarray(enc.numpy(), dtype=np.float32).reshape(-1)
+    n = min(e.size, 1 << 22)  # 16 MB of float32
+    idx = np.sort(np.random.default_rng(1234).integers(0, e.size, n)) if n < e.size else np.arange(e.size)
+    np.save(os.path.join(d, f"{workload}_encoder_output_sample.npy"), e[idx])
 
 
 def enc_flops_per_chunk(dims) -> float:
@@ -411,6 +406,8 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--cpu-sample-tokens", type=int, default=32)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

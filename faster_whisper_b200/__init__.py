@@ -1,4 +1,4 @@
-"""B200-native Whisper engine with faster-whisper's public API (reference ``faster_whisper/__init__.py:1-14``)."""
+"""Hopper (H100) Whisper engine with faster-whisper's public API (reference ``faster_whisper/__init__.py:1-14``)."""
 
 from .audio import decode_audio
 from .transcribe import BatchedInferencePipeline, WhisperModel

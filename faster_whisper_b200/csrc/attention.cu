@@ -1,12 +1,11 @@
-// Encoder self-attention (non-causal, T = 1500, head_dim = 64) as a flash-attention forward on tcgen05.
+// Encoder self-attention (non-causal, T = 1500, head_dim = 64) as a flash-attention forward on Hopper wgmma.
 //
-// One CTA per (128-query tile, head, chunk).  TMA streams Q once and K/V tiles of 128 keys through a
-// 2-deep ring; S = Q K^T lands in TMEM (UMMA 128x128x16), four softmax warps own one query row per thread
-// (TMEM lane == row, so row max / row sum need no shuffles), write P as packed fp16 back into TMEM, and
-// P V runs as a TMEM-A / shared-memory-B UMMA (128x64x16, V consumed MN-major straight from the fused QKV
-// activation layout — no transpose pass).  The running output is rescaled in registers (online softmax).
-// Two CTAs co-reside per SM (80 KB smem, 256 TMEM columns each) so one CTA's exponentials overlap the
-// other's MMAs.
+// One CTA per (128-query tile, head, chunk).  A producer warp streams Q once and K/V tiles of 128 keys through a
+// 2-deep TMA ring; two consumer warpgroups own 64 query rows each.  S = Q K^T is one wgmma chain (m64n128k16,
+// both operands in shared memory, accumulators in registers); the online softmax runs on those registers (a row is
+// spread over the four threads of a quad, so row max / row sum take two shuffles), P is rounded to fp16 in registers
+// and fed straight back as the A operand of P V (m64n64k16, V consumed MN-major from the fused QKV activation layout
+// — no transpose pass).  The running output is rescaled in registers before each P V chain accumulates into it.
 //
 // Replaces CTranslate2's batched-GEMM + softmax kernel + batched-GEMM attention (SURVEY.md §2.3 row K5)
 // inside Whisper.encode (reference faster_whisper/transcribe.py:1391-1400).
@@ -14,19 +13,16 @@
 
 #include "common.cuh"
 #include "engine.h"
+#include "wgmma.cuh"
 
 namespace b2w {
 
-constexpr int kAttnThreads = 192;
+constexpr int kAttnThreads = 288;         // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int kTileBytes = 128 * 64 * 2;  // 16 KB: 128 rows x 64 halves, 128B-swizzled
 constexpr int kKvStages = 2;
 
-__global__ void __launch_bounds__(kAttnThreads, 2)
+__global__ void __launch_bounds__(kAttnThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tm, __half* __restrict__ out, int T, int H) {
-  constexpr uint32_t IDESC_S = umma_idesc_f16(128, 128, false);
-  constexpr uint32_t IDESC_O = umma_idesc_f16(128, 64, true);
-  constexpr int TMEM_COLS = 256;  // S: [0,128)  P(fp16x2): [128,192)  O_tile: [192,256)
-
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -35,10 +31,6 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, __half* __restrict__ out,
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;
   uint64_t* kv_empty = kv_full + kKvStages;
-  uint64_t* s_full = kv_empty + kKvStages;
-  uint64_t* p_full = s_full + 1;
-  uint64_t* o_full = p_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
@@ -49,21 +41,13 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, __half* __restrict__ out,
     mbar_init(q_full, 1);
     for (int i = 0; i < kKvStages; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&kv_empty[i], 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tP = tmem_base + 128, tO = tmem_base + 192;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       tma_prefetch_desc(&tm);
       mbar_expect_tx(q_full, kTileBytes);
@@ -77,105 +61,98 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tm, __half* __restrict__ out,
         tma_load_3d(k_dst + kTileBytes, &tm, &kv_full[s], 2 * d + h * 64, j * 128, b);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(q_full, 0);
-      const uint64_t dq = umma_smem_desc_sw128(smem_u32(sQ));
-      for (int j = 0; j < n_kv; ++j) {
-        const int s = j % kKvStages;
-        mbar_wait(&kv_full[s], (j / kKvStages) & 1);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(sKV + s * 2 * kTileBytes);
-        const uint64_t dk = umma_smem_desc_sw128(k_addr);
-        const uint64_t dv = umma_smem_desc_sw128(k_addr + kTileBytes);
+    return;
+  }
+
+  const int wg = warp >> 2, wq = warp & 3, tig = threadIdx.x & 127;
+  const int g = lane >> 2, t = lane & 3;
+  const float sc = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // rows g and g + 8 of this warp's 16; l: this thread's columns only
+  float o[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_ss(tS, dq + 2 * k, dk + 2 * k, IDESC_S, k != 0 ? 1u : 0u);
-        tc_commit(s_full);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  mbar_wait(q_full, 0);
+  const uint64_t dq = wgmma_desc_sw128(smem_u32(sQ) + wg * (64 * 128));
+  for (int j = 0; j < n_kv; ++j) {
+    const int s = j % kKvStages;
+    mbar_wait(&kv_full[s], (j / kKvStages) & 1);
+    const uint32_t k_addr = smem_u32(sKV + s * 2 * kTileBytes);
+    const uint64_t dk = wgmma_desc_sw128(k_addr);
+    const uint64_t dv = wgmma_desc_sw128(k_addr + kTileBytes);
+    float sacc[64];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) umma_ts(tO, tP + 8 * k, dv + k * (2048 >> 4), IDESC_O, k != 0 ? 1u : 0u);
-        tc_commit(o_full);
-        tc_commit(&kv_empty[s]);
+    for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss_n128(sacc, dq + 2 * k, dk + 2 * k, 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int kbase = j * 128 + 2 * t;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if (kbase + 8 * i + (e & 1) >= T) sacc[4 * i + e] = -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], sacc[4 * i + e]);
       }
     }
-  } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_off = uint32_t(q * 32) << 16;
-    const float sc = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-    float m_run = -INFINITY, l_run = 0.f;
-    float o[64];
+    float alpha[2], m_new[2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] = 0.f;
-    for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      const int kbase = j * 128;
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tS + lane_off + c * 32, v);
-        tc_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (kbase + c * 32 + i < T) mx = fmaxf(mx, __uint_as_float(v[i]));
-      }
-      const float m_new = fmaxf(m_run, mx * sc);
-      const float alpha = (m_run == -INFINITY) ? 0.f : ex2_approx(m_run - m_new);
-      float l_new = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tS + lane_off + c * 32, v);
-        tc_wait_ld();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float p0 = (kbase + c * 32 + 2 * i < T) ? ex2_approx(__uint_as_float(v[2 * i]) * sc - m_new) : 0.f;
-          float p1 = (kbase + c * 32 + 2 * i + 1 < T) ? ex2_approx(__uint_as_float(v[2 * i + 1]) * sc - m_new) : 0.f;
-          const __half2 hh = __floats2half2_rn(p0, p1);
-          // the row sum uses the rounded probabilities that the P*V product will see
-          l_new += __low2float(hh) + __high2float(hh);
-          pk[i] = *reinterpret_cast<const uint32_t*>(&hh);
-        }
-        tmem_st16(tP + lane_off + c * 16, pk);
-      }
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(p_full);
-      mbar_wait(o_full, j & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tO + lane_off + c * 32, v);
-        tc_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[c * 32 + i] = fmaf(o[c * 32 + i], alpha, __uint_as_float(v[i]));
-      }
-      l_run = fmaf(l_run, alpha, l_new);
-      m_run = m_new;
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      m_new[r] = fmaxf(m_run[r], mx[r] * sc);
+      alpha[r] = (m_run[r] == -INFINITY) ? 0.f : ex2_approx(m_run[r] - m_new[r]);
+      m_run[r] = m_new[r];
     }
-    if (q0 + row < T) {
-      const float inv = 1.0f / l_run;
-      uint4* dst = reinterpret_cast<uint4*>(out + ((long long)b * T + q0 + row) * d + h * 64);
+    // P as fp16 A fragments: k-step kk covers keys 16 kk .. 16 kk + 15 = accumulator column blocks 2 kk and 2 kk + 1
+    uint32_t pa[8][4];
+    float l_new[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float p0 = ex2_approx(sacc[4 * i + 2 * r] * sc - m_new[r]);  // masked keys: ex2(-inf) = 0
+        const float p1 = ex2_approx(sacc[4 * i + 2 * r + 1] * sc - m_new[r]);
+        const __half2 hh = __floats2half2_rn(p0, p1);
+        // the row sum uses the rounded probabilities that the P*V product will see
+        l_new[r] += __low2float(hh) + __high2float(hh);
+        pa[i >> 1][(i & 1) * 2 + r] = *reinterpret_cast<const uint32_t*>(&hh);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i] *= alpha[0];
+      o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1];
+      o[4 * i + 3] *= alpha[1];
+    }
+    l_run[0] = fmaf(l_run[0], alpha[0], l_new[0]);
+    l_run[1] = fmaf(l_run[1], alpha[1], l_new[1]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64_t(o, pa[kk], dv + kk * (2048 >> 4), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (tig == 0) mbar_arrive(&kv_empty[s]);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    const int row = q0 + wg * 64 + wq * 16 + g + 8 * r;
+    if (row < T) {
+      const float inv = 1.0f / l_run[r];
+      __half* dst = out + ((long long)b * T + row) * d + h * 64 + 2 * t;
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        dst[i] = make_uint4(pack_half2(o[8 * i] * inv, o[8 * i + 1] * inv), pack_half2(o[8 * i + 2] * inv, o[8 * i + 3] * inv),
-                            pack_half2(o[8 * i + 4] * inv, o[8 * i + 5] * inv), pack_half2(o[8 * i + 6] * inv, o[8 * i + 7] * inv));
+        *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_half2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
-static int attn_smem_bytes() { return kTileBytes * (1 + 2 * kKvStages) + 1024 + 128; }
+static int attn_smem_bytes() { return kTileBytes * (1 + 2 * kKvStages) + 1024 + 64; }
 
 AttnPlan attn_plan(const __half* qkv, __half* out, int B, int T, int H) {
   AttnPlan p;

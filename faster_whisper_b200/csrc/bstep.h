@@ -4,8 +4,9 @@
 
 namespace b2w {
 
-constexpr int kBsAtomBytes = 16384;  // one weight atom: 128 output channels x 64 K values, fp16, 128-byte swizzle (a ready-made UMMA A tile)
+constexpr int kBsAtomBytes = 16384;  // one weight atom: 128 output channels x 64 K values, fp16, 128-byte swizzle (a ready-made wgmma A tile)
 constexpr int kBsMaxRows = 80;
+constexpr int kBsBarWords = 64 + 6 * 64;
 
 // Per layer: the six weight matrices as atom streams (order: qkv, out, cross_q, cross_out, ffn1, ffn2), their fp32 biases and, for the
 // three matrices that consume a LayerNorm, the row sums of the (LayerNorm-folded, fp16-rounded) weights — the mean term of the
@@ -25,21 +26,23 @@ struct BStepArgs {
   const void* logit_atoms;    // (LayerNorm-folded) output embedding as an atom stream, rows padded to a multiple of 128
   const float* logit_bias;    // [vpad]
   const float* logit_scale;   // [vpad] (w8)
-  int w8;                     // 1: int8 atom streams, widened to fp16 UMMA tiles in shared memory by the compute warps
-  int R, NP;                  // rows, rows padded to the UMMA N (multiple of 16)
+  int w8;                     // 1: int8 atom streams, widened to fp16 wgmma tiles in shared memory by the compute warps
+  int R, NP;                  // rows, rows padded to the wgmma N (multiple of 16)
   int d, H, n_ctx, slots, T, vpad, n_vocab, n_chunks, rows_per_chunk;
   int u_bytes;                // size of the multi-purpose shared-memory region
   int stop_phase;             // debug: number of grid phases to run (<= 0: all)
   const RowInfo* rows;
   const int* tokens_in;
   float* x;       // [R][d]   fp32 residual stream
-  float* qkv32;   // [R][3d]  raw W_qkv x (split-K sums, reduced in L2)
+  float* qkv32;   // [R][3d]  raw W_qkv x (split-K sums, reduced in a fixed order)
   float* cq32;    // [R][d]   raw cross-attention query
   float* h32;     // [R][4d]  raw FFN hidden
   __half* ao;     // [R][d]   attention output
   __half* h16;    // [R][4d]  GELU(hidden)
   __half* xn16;   // [R][d]   final LayerNorm output
   float* stats;   // [3L][R][2]  sum(x), sum(x^2) of the residual stream at each LayerNorm
+  float* stpart;  // [d/64][R][2] per-k-atom partials of the statistics of the current GEMM phase
+  float* gpart;   // [grid][R][128] each CTA's split-K partial tile of the current GEMM phase
   float* logits;  // [R][vpad]
   __half* kcache;
   __half* vcache;
@@ -49,7 +52,7 @@ struct BStepArgs {
   const DecBindings* bind;
   float* xpart;
   int* xcounters;
-  unsigned* bar;
+  unsigned* bar;  // [kBsBarWords]: grid barrier, then from word 64 the n-block group counters [6 matrices][64 n-blocks]
   unsigned long long* prof;  // optional: %globaltimer at every barrier (CTA 0)
 };
 

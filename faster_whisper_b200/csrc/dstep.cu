@@ -3,7 +3,7 @@
 // With so few rows every sub-layer streams 3-13 MB of weights: as separate launches each costs 6-15 us, and a large-v3
 // step is 257 of them.  Here one CTA per SM stays resident for the whole step and walks the phases
 //   embed | L x { QKV, self-attn, out-proj, cross-q, cross-attn, cross-out, FFN1, FFN2 } | logits
-// separated by grid barriers.  What shapes it (measured on B200: tools/bench/*.cu, profiles/r1_dstep_*.txt):
+// separated by grid barriers.  What shapes it (orders of magnitude; tools/bench/*.cu measures them on the GPU at hand):
 //   * a dependent hop through L2 costs ~0.6 us and a grid barrier ~1.4 us, so a phase has a ~2.4 us floor.  Everything a
 //     phase needs that does not depend on the previous phase is therefore fetched ahead of time: the weights are stored as
 //     a stream of per-work-item tiles (dstep_pack_tiles) and a three-deep shared-memory ring is kept full across phase

@@ -4,7 +4,7 @@
 
 namespace b2w {
 
-constexpr int kDsXSplits = 7;    // key splits of the beam-shared cross attention (20 heads x 7 = 140 tasks for 148 SMs)
+constexpr int kDsXSplits = 7;    // key splits of the beam-shared cross attention (20 heads x 7 = 140 tasks, about one per SM)
 constexpr int kDsXKeysMax = 224;  // keys per cross-attention tile (multiple of 16, >= ceil(T / kDsXSplits) + 1)
 
 // Per layer: the six weight matrices of the step re-laid out as a stream of work-item tiles (dstep_pack_tiles), in the order

@@ -1,6 +1,6 @@
 // Host-side engine: weight upload, encoder orchestration, generate loop, and the extern "C" ABI declared in
 // include/b200whisper.h.  PyTorch is not involved: the library owns its device memory and one CUDA stream per
-// model.  There is no CPU fallback — every entry point fails loudly when no sm_100 device is usable.
+// model.  There is no CPU fallback — every entry point fails loudly when no sm_90 device is usable.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -42,7 +42,7 @@ struct DeviceGuard {
   ~DeviceGuard() { cudaSetDevice(prev); }
 };
 
-static void require_blackwell(int device) {
+static void require_hopper(int device) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n == 0)
@@ -50,7 +50,7 @@ static void require_blackwell(int device) {
   if (device < 0 || device >= n) throw Error("device index out of range", true);
   cudaDeviceProp prop;
   B2W_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) throw Error(std::string("device ") + prop.name + " is not sm_100 (Blackwell); kernels are sm_100a only");
+  if (prop.major != 9 || prop.minor != 0) throw Error(std::string("device ") + prop.name + " is not sm_90 (Hopper); kernels are sm_90a only");
 }
 
 template <typename T>
@@ -66,7 +66,7 @@ Model::~Model() {
   for (void* p : allocs) cudaFree(p);
   for (auto& it : pool) cudaFree(it.second);
   void* ws[] = {e_feats, e_x0, e_x1, e_x, e_xn, e_qkv, e_ao, e_h, e_pcm, e_chunks, e_chunk_max, kcache, vcache, d_x, d_xn,
-                d_q, d_ao, d_h, d_logits, d_xpart, d_counters, d_suppress, sb_blob, d_bind, d_layers, d_bar};
+                d_q, d_ao, d_h, d_logits, d_xpart, d_counters, d_suppress, sb_blob, d_bind, d_layers, d_bar, d_gpart, d_stpart};
   for (void* p : ws)
     if (p) cudaFree(p);
   if (h_pinned) cudaFreeHost(h_pinned);
@@ -533,8 +533,8 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
       B2W_CUDA(cudaMemcpy(m->d_blayers, bl.data(), L * sizeof(BLayer), cudaMemcpyHostToDevice));
       m->bstep_packed = true;
     }
-    m->d_bar = dalloc<unsigned>(4);
-    B2W_CUDA(cudaMemset(m->d_bar, 0, 4 * sizeof(unsigned)));
+    m->d_bar = dalloc<unsigned>(kBsBarWords);
+    B2W_CUDA(cudaMemset(m->d_bar, 0, kBsBarWords * sizeof(unsigned)));
   }
   for (int l = L / 2; l < L; ++l)  // default alignment heads: every head of the last half of the decoder (OpenAI Whisper's default)
     for (int hh = 0; hh < cfg.n_text_head; ++hh) m->align_heads.push_back(make_int2(l, hh));
@@ -721,6 +721,8 @@ static void ensure_decoder_ws(Model* m, int chunks, int slots) {
     m->d_h16 = dalloc<__half>((size_t)kMaxRows * 4 * dt);
     m->d_xn16 = dalloc<__half>((size_t)kMaxRows * dt);
     m->d_stats = dalloc<float>((size_t)3 * L * kMaxRows * 2 + 4);
+    m->d_gpart = dalloc<float>((size_t)m->num_sms * kMaxRows * 128);  // the many-row step kernel's per-CTA split-K partial tiles
+    m->d_stpart = dalloc<float>((size_t)(dt / 64) * kMaxRows * 2);
     B2W_CUDA(cudaMemset(m->d_xn, 0, (size_t)kMaxRows * dt * 2));
     B2W_CUDA(cudaMemset(m->d_ao, 0, (size_t)kMaxRows * dt * 2));
     B2W_CUDA(cudaMemset(m->d_h, 0, (size_t)kMaxRows * 4 * dt * 2));
@@ -821,7 +823,7 @@ static void ensure_cross_kv(Model* m, Encoded* e) {
   }
 }
 
-constexpr int kTcMinRows = 17;  // rows above which the decode GEMMs go through the tcgen05 path (activations reused from smem)
+constexpr int kTcMinRows = 17;  // rows above which the decode GEMMs go through the wgmma path (activations reused from smem)
 
 // decode GEMM through the tensor-core GEMM: the plan (TMA maps) is cached per (weights, activations, rows)
 static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
@@ -854,11 +856,8 @@ static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
     case GV_F16: g.epilogue = EPI_F16; g.out = a.out_h; g.out_ld = a.N; break;
     case GV_GELU_F16: g.epilogue = EPI_GELU_F16; g.out = a.out_h; g.out_ld = a.N; break;
     case GV_RESID_LN: {
-      // x += y W^T: four K ranges reduced in place with fp32 atomics when the K blocks allow it (more CTAs streaming the weights)
-      const int num_kb = a.K / 64;
-      const int ks = num_kb % 4 == 0 ? 4 : (num_kb % 2 == 0 ? 2 : 1);
-      g.epilogue = ks > 1 ? EPI_RESID_ATOMIC : EPI_RESID_F32;
-      g.ksplit = ks;
+      // x += y W^T in place: every element is written by the one tile that holds all of its K (no atomics: the same bits every run)
+      g.epilogue = EPI_RESID_F32;
       g.out = a.xres; g.resid = a.xres; g.out_ld = a.N;
       break;
     }
@@ -1131,7 +1130,7 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
     if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // re-read per call: tools/bstep_bisect.py steps it
     bs.rows = sb.rows; bs.tokens_in = sb.tokens_in;
     bs.x = m->d_x; bs.qkv32 = m->d_qkv32; bs.cq32 = m->d_cq32; bs.h32 = m->d_h32; bs.ao = m->d_ao; bs.h16 = m->d_h16; bs.xn16 = m->d_xn16;
-    bs.stats = m->d_stats; bs.logits = m->d_logits;
+    bs.stats = m->d_stats; bs.stpart = m->d_stpart; bs.gpart = m->d_gpart; bs.logits = m->d_logits;
     bs.kcache = m->kcache; bs.vcache = m->vcache; bs.kv_layer_stride = (long long)m->kv_elems;
     bs.anc = sb.anc; bs.anc_buf_stride = (long long)n * K * c.n_text_ctx;
     bs.bind = m->d_bind; bs.xcounters = m->d_counters + 64; bs.bar = m->d_bar; bs.prof = m->d_prof;
@@ -1276,8 +1275,8 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
         for (int k = 0; k < 6; ++k) {
           const double cnt = (double)f[k * 16 + 15];
           if (cnt > 0)
-            fprintf(stderr, "[bstep prof]   %-9s cycles (CTA 0): stage %.0f  sync %.0f  row statistics %.0f  mma-wait %.0f  epilogue %.0f  bulk-wait %.0f\n", kinds[k],
-                    f[k * 16] / cnt, f[k * 16 + 4] / cnt, f[k * 16 + 5] / cnt, f[k * 16 + 1] / cnt, f[k * 16 + 2] / cnt, f[k * 16 + 3] / cnt);
+            fprintf(stderr, "[bstep prof]   %-9s cycles (CTA 0): stage %.0f  sync %.0f  row statistics %.0f  products + reduction %.0f\n", kinds[k],
+                    f[k * 16] / cnt, f[k * 16 + 4] / cnt, f[k * 16 + 5] / cnt, f[k * 16 + 2] / cnt);
         }
       }
     }
@@ -1405,7 +1404,7 @@ int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n
                      const char* compute_type, b2w_model** out) {
   return guarded([&] {
     B2W_CHECK(cfg && tensors && out, "null argument");
-    require_blackwell(device);
+    require_hopper(device);
     const std::string ct = compute_type ? compute_type : "default";
     const char* ok[] = {"default", "auto", "float16", "int8_float16", "int8", "float32", "bfloat16", "int8_float32", "int8_bfloat16", "int16"};
     bool known = false;
@@ -1478,7 +1477,7 @@ int b2w_logmel(int32_t device, int32_t n_mels, const float* pcm, int64_t n_sampl
                int64_t out_capacity, int32_t* n_frames_out) {
   return guarded([&] {
     B2W_CHECK(n_mels > 0 && n_mels <= 128 && n_samples >= 0 && padding >= 0, "bad log-mel arguments");
-    require_blackwell(device);
+    require_hopper(device);
     DeviceGuard g(device);
     static thread_local std::map<std::pair<int, int>, std::unique_ptr<MelPlan>> plans;
     auto& plan = plans[{device, n_mels}];
@@ -1953,7 +1952,7 @@ int b2w_counters_get(b2w_model* h, int64_t* launches, int64_t* decode_steps, dou
 int b2w_debug_gemm(int32_t device, int32_t impl, const float* a, const float* w, const float* bias, int32_t M, int32_t N,
                    int32_t K, int32_t gelu, float* c_out) {
   return guarded([&] {
-    require_blackwell(device);
+    require_hopper(device);
     DeviceGuard g(device);
     cudaDeviceProp prop;
     B2W_CUDA(cudaGetDeviceProperties(&prop, device));
@@ -1989,7 +1988,7 @@ int b2w_debug_gemm(int32_t device, int32_t impl, const float* a, const float* w,
 
 int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t B, int32_t T, int32_t H, float* out) {
   return guarded([&] {
-    require_blackwell(device);
+    require_hopper(device);
     DeviceGuard g(device);
     const size_t n_in = (size_t)B * T * 3 * H * 64, n_out = (size_t)B * T * H * 64;
     float *dq = dalloc<float>(n_in), *dof = dalloc<float>(n_out);
@@ -2012,7 +2011,7 @@ int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t 
 int b2w_debug_gemv(int32_t device, int32_t impl, const float* x, const float* w, const float* bias, int32_t R, int32_t N,
                    int32_t K, float* y_out) {
   return guarded([&] {
-    require_blackwell(device);
+    require_hopper(device);
     DeviceGuard g(device);
     const int Np = ceil_div(N, 16) * 16, Rp = ceil_div(R, 8) * 8;
     float *dx = dalloc<float>((size_t)Rp * K), *dw = dalloc<float>((size_t)Np * K), *db = dalloc<float>(Np), *dy = dalloc<float>((size_t)R * Np);

@@ -27,7 +27,7 @@ struct MelPlan {
            int out_ld, int* chunk_max_dev, bool zero_fill, cudaStream_t stream) const;
 };
 
-// ---- dense GEMM on tcgen05 (gemm.cu) --------------------------------------------------------------------
+// ---- dense GEMM on wgmma (gemm.cu) --------------------------------------------------------------------
 enum Epilogue {
   EPI_F16 = 0,           // out(f16) = acc + bias
   EPI_GELU_F16 = 1,      // out(f16) = gelu(acc + bias)
@@ -36,7 +36,6 @@ enum Epilogue {
   EPI_F16_XKV = 4,       // cross-KV scatter: out[l][kv][b][h][t][64] (f16) = acc + bias
   EPI_F32 = 5,           // out(f32) = acc + bias
   EPI_QKV_CACHE = 6,     // decoder fused QKV: q -> out(f16)[row][d]; k,v -> paged self-KV cache at (chunk,pos,slot) of the row
-  EPI_RESID_ATOMIC = 7,  // out(f32) += acc (+ bias on the first K split): split-K partial sums reduced in place with fp32 vector atomics
 };
 
 struct GemmArgs {
@@ -62,16 +61,15 @@ struct GemmArgs {
   __half* vcache = nullptr;
   int qkv_d = 0, n_ctx = 0, slots = 0;
   int epilogue = EPI_F16;
-  // few-row GEMMs (decode rows): prefer narrow 32-column tiles and `ksplit` K ranges so that more than N/128 CTAs stream the weights
+  // few-row GEMMs (decode rows): prefer narrow 32-column tiles so that more than N/128 CTAs stream the weights
   bool narrow_tiles = false;
-  int ksplit = 1;  // > 1 only with EPI_RESID_ATOMIC
 };
 
 struct GemmPlan {
   GemmArgs a;
   CUtensorMap tmA, tmB;
   int block_n = 128;
-  int tiles_m = 0, tiles_n = 0, num_kb = 0, grid = 0, ksplit = 1;
+  int tiles_m = 0, tiles_n = 0, num_kb = 0, grid = 0;
   double flops() const { return 2.0 * a.a_batch * a.rows * (double)a.N * a.taps * a.k_per_tap; }
 };
 GemmPlan gemm_plan(const GemmArgs& a, int num_sms);
@@ -79,7 +77,7 @@ void gemm_run(const GemmPlan& p, cudaStream_t stream);
 void gemm_configure();  // per-device kernel attributes; call once per device outside stream capture
 void gemm_ref_run(const GemmArgs& a, cudaStream_t stream);  // plain SIMT reference of the same contract
 
-// ---- encoder attention on tcgen05 (attention.cu) ---------------------------------------------------------
+// ---- encoder attention on wgmma (attention.cu) ---------------------------------------------------------
 struct AttnPlan {
   const __half* qkv = nullptr;  // [B][T][3*H*64]
   __half* out = nullptr;        // [B][T][H*64]

@@ -1,25 +1,27 @@
 // Dense GEMM C[M,N] = epilogue(A[M,K] * W[N,K]^T) for the Whisper encoder, the conv stem (implicit GEMM with
 // K-block -> tap mapping done by TMA coordinates) and the cross-KV projection.
 //
-// sm_100a only: operands move HBM -> shared memory with TMA (128-byte swizzle, 64-wide K blocks), the
-// product runs on the 5th-gen tensor cores with tcgen05.mma (UMMA 128 x BN x 16, fp16 in, fp32 accumulate)
-// issued by one elected thread, accumulators live in TMEM (double buffered so the epilogue of tile i overlaps
-// the MMAs of tile i+1), and the bias / GELU / residual / position-add / layout-scatter epilogues are fused
-// on the TMEM -> register path (tcgen05.ld).  Persistent CTAs, one per SM, static tile scheduler.
+// sm_90a: operands move HBM -> shared memory with TMA (128-byte swizzle, 64-wide K blocks) through a ring of stages fed by
+// one producer warp; two consumer warpgroups each own 64 rows of the 128-row tile and run the product on the Hopper tensor
+// cores with wgmma.mma_async (m64 x {32,128} x k16, fp16 in, fp32 accumulators in registers), one wgmma group in flight while
+// the stage of the previous one is handed back to the producer.  The bias / GELU / residual / position-add /
+// layout-scatter epilogues are fused: each warpgroup passes its accumulators through a small shared-memory tile so that
+// a thread stores 32 consecutive columns of one row.  Persistent CTAs, one per SM, static tile scheduler.
 //
 // Replaces what CTranslate2 does with cuBLAS GEMM + cuDNN conv + separate bias/GELU/add kernels
 // (SURVEY.md §2.3 rows K1-K9) behind Whisper.encode (reference faster_whisper/transcribe.py:1391-1400).
 #include "common.cuh"
 #include "engine.h"
+#include "wgmma.cuh"
 
 namespace b2w {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int kGemmThreads = 192;  // warp0: TMA, warp1: MMA + TMEM alloc, warps 2-5: epilogue
+constexpr int kGemmThreads = 288;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 
 struct GemmDev {
-  int batch, tiles_m, tiles_n, num_kb, kb_per_tap, ksplit;
+  int batch, tiles_m, tiles_n, num_kb, kb_per_tap;
   int tap_row[3], tap_col[3];
   int rows, N;
   const float* bias;
@@ -35,11 +37,11 @@ struct GemmDev {
 };
 
 template <int EPI>
-__device__ __forceinline__ void epilogue_store(const GemmDev& p, int b, int row, int n0, const uint32_t* vraw, bool with_bias) {
+__device__ __forceinline__ void epilogue_store(const GemmDev& p, int b, int row, int n0, const float* vin) {
   float v[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(vraw[i]);
-  if (p.bias && with_bias) {
+  for (int i = 0; i < 32; ++i) v[i] = vin[i];
+  if (p.bias) {
     const float4* b4 = reinterpret_cast<const float4*>(p.bias + n0);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -94,10 +96,7 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, int b, int row,
   } else {
     const long long idx = (long long)b * p.out_batch_stride + (long long)row * p.out_ld + n0;
     float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + idx);
-    if constexpr (EPI == EPI_RESID_ATOMIC) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) atomicAdd(o4 + i, make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]));
-    } else if constexpr (EPI == EPI_RESID_F32) {
+    if constexpr (EPI == EPI_RESID_F32) {
       const float4* r4 = reinterpret_cast<const float4*>(p.resid + idx);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -118,56 +117,52 @@ __device__ __forceinline__ void epilogue_store(const GemmDev& p, int b, int row,
   }
 }
 
+template <int BN>
+struct GemmCfg {
+  static constexpr int STAGES = BN == 128 ? 6 : 8;
+  static constexpr int A_BYTES = BM * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int EC = BN < 64 ? BN : 64;  // epilogue columns per pass through shared memory
+  static constexpr int EC4 = EC / 4;          // 16-byte chunks per epilogue row, stored at chunk ^ (row % EC4) (no bank conflicts)
+  static constexpr int EPI_BYTES = 2 * 64 * EC * 4;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+};
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
-  constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  constexpr int A_BYTES = BM * BK * 2;
-  constexpr int B_BYTES = BN * BK * 2;
-  constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t IDESC = umma_idesc_f16(BM, BN, false);
-  constexpr int TMEM_COLS = 2 * BN;  // 64, 256 or 512: two accumulator buffers
+  using C = GemmCfg<BN>;
+  constexpr int STAGES = C::STAGES, A_BYTES = C::A_BYTES, STAGE_BYTES = C::STAGE_BYTES, EC = C::EC, EC4 = C::EC4;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  float* epi = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + C::EPI_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 128);
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int total_tiles = p.batch * p.tiles_m * p.tiles_n * p.ksplit;  // tile = ((b * tiles_m + m) * tiles_n + n) * ksplit + ks
+  const int total_tiles = p.batch * p.tiles_m * p.tiles_n;  // tile = (b * tiles_m + m) * tiles_n + n
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       tma_prefetch_desc(&tmA);
       tma_prefetch_desc(&tmB);
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int ks = tile % p.ksplit, t2 = tile / p.ksplit;
-        const int n_idx = t2 % p.tiles_n;
-        const int rest = t2 / p.tiles_n;
+        const int n_idx = tile % p.tiles_n;
+        const int rest = tile / p.tiles_n;
         const int m_idx = rest % p.tiles_m, b = rest / p.tiles_m;
-        const int kb0 = ks * p.num_kb / p.ksplit, kb1 = (ks + 1) * p.num_kb / p.ksplit;
-        for (int kb = kb0; kb < kb1; ++kb) {
+        for (int kb = 0; kb < p.num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           const int tap = kb / p.kb_per_tap, kc = kb - tap * p.kb_per_tap;
@@ -181,82 +176,77 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        const int ks = tile % p.ksplit;
-        const int kb0 = ks * p.num_kb / p.ksplit, kb1 = (ks + 1) * p.num_kb / p.ksplit;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint64_t da = umma_smem_desc_sw128(sa);
-          const uint64_t db = umma_smem_desc_sw128(sa + A_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_ss(d_tmem, da + 2 * k, db + 2 * k, IDESC, (kb != kb0 || k != 0) ? 1u : 0u);
-          tc_commit(&empty[stage]);  // frees the smem slot once these MMAs retire
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tc_commit(&tfull[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
-    const int row_in_tile = q * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int ks = tile % p.ksplit, t2 = tile / p.ksplit;
-      const int n_idx = t2 % p.tiles_n;
-      const int rest = t2 / p.tiles_n;
-      const int m_idx = rest % p.tiles_m, b = rest / p.tiles_m;
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const int row = m_idx * BM + row_in_tile;
-      const bool valid = row < p.rows;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + (uint32_t(q * 32) << 16) + acc * BN + c0, v);
-        tc_wait_ld();
-        const int n0 = n_idx * BN + c0;
-        if (valid && n0 < p.N) epilogue_store<EPI>(p, b, row, n0, v, ks == 0);
-      }
-      tc_fence_before();
-      mbar_arrive(&tempty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+
+  const int wg = warp >> 2, wq = warp & 3, tig = threadIdx.x & 127;
+  const int g = lane >> 2, t = lane & 3;
+  float* my_epi = epi + wg * 64 * EC;
+  const uint32_t bar_id = 1 + wg;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int n_idx = tile % p.tiles_n;
+    const int rest = tile / p.tiles_n;
+    const int m_idx = rest % p.tiles_m, b = rest / p.tiles_m;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < p.num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+      const uint64_t da = wgmma_desc_sw128(sa + wg * (64 * 128));
+      const uint64_t db = wgmma_desc_sw128(sa + A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, 1);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's products are done: hand its slot back
+      if (prev >= 0 && tig == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && tig == 0) mbar_arrive(&empty[prev]);
+
+    const int row_l = tig & 63, half = tig >> 6;
+    const int row = m_idx * BM + wg * 64 + row_l;
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += EC) {
+#pragma unroll
+      for (int i = c0 / 8; i < (c0 + EC) / 8; ++i) {
+        const int col = 8 * i + 2 * t - c0, r = 16 * wq + g;
+        const int c4 = col >> 2, cw = col & 3;
+        *reinterpret_cast<float2*>(my_epi + r * EC + ((c4 ^ (r % EC4)) << 2) + cw) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(my_epi + (r + 8) * EC + ((c4 ^ ((r + 8) % EC4)) << 2) + cw) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+      const int n0 = n_idx * BN + c0 + half * 32;
+      if (half * 32 < EC && row < p.rows && n0 < p.N) {
+        float v[32];
+        const float4* src = reinterpret_cast<const float4*>(my_epi + row_l * EC);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 f = src[(half * 8 + i) ^ (row_l % EC4)];
+          v[4 * i] = f.x;
+          v[4 * i + 1] = f.y;
+          v[4 * i + 2] = f.z;
+          v[4 * i + 3] = f.w;
+        }
+        epilogue_store<EPI>(p, b, row, n0, v);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+    }
   }
 }
 
 template <int BN>
 static int gemm_smem_bytes() {
-  constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  return STAGES * (BM * BK * 2 + BN * BK * 2) + 1024 /*align slack*/ + 256 /*barriers*/;
+  return GemmCfg<BN>::SMEM;
 }
 
 GemmPlan gemm_plan(const GemmArgs& a, int num_sms) {
@@ -267,18 +257,14 @@ GemmPlan gemm_plan(const GemmArgs& a, int num_sms) {
   p.a = a;
   const int K = a.taps * a.k_per_tap;
   p.tiles_m = ceil_div(a.rows, BM);
-  long long tiles256 = (long long)a.a_batch * p.tiles_m * ceil_div(a.N, 256);
-  p.block_n = (a.N % 256 == 0 && tiles256 >= 2LL * num_sms) ? 256 : 128;
+  // 128 x 128 tiles: a 256-wide tile needs 128 accumulator registers per consumer thread, more than the 168 a 288-thread CTA may
+  // hold next to the epilogue
+  p.block_n = 128;
   // few rows (one M tile): a 128-wide tiling leaves most SMs without work while the weights stream through N/128 CTAs
   if (a.narrow_tiles && a.a_batch * p.tiles_m == 1 && ceil_div(a.N, 128) * 2 <= num_sms) p.block_n = 32;
   p.tiles_n = ceil_div(a.N, p.block_n);
   p.num_kb = K / BK;
-  p.ksplit = 1;
-  if (a.epilogue == EPI_RESID_ATOMIC) {
-    B2W_CHECK(a.ksplit >= 1 && p.num_kb % a.ksplit == 0, "GEMM K split must divide the K blocks");
-    p.ksplit = a.ksplit;
-  }
-  long long total = (long long)a.a_batch * p.tiles_m * p.tiles_n * p.ksplit;
+  long long total = (long long)a.a_batch * p.tiles_m * p.tiles_n;
   p.grid = (int)(total < num_sms ? total : num_sms);
   {
     uint64_t dims[3] = {(uint64_t)a.a_cols, (uint64_t)a.a_rows, (uint64_t)a.a_batch};
@@ -314,12 +300,10 @@ static void configure_bn() {
   configure_one<BN, EPI_F16_XKV>();
   configure_one<BN, EPI_F32>();
   configure_one<BN, EPI_QKV_CACHE>();
-  configure_one<BN, EPI_RESID_ATOMIC>();
 }
 void gemm_configure() {
   configure_bn<32>();
   configure_bn<128>();
-  configure_bn<256>();
 }
 
 template <int BN>
@@ -332,14 +316,12 @@ static void dispatch_epi(const GemmPlan& pl, const GemmDev& d, cudaStream_t s) {
     case EPI_F16_XKV: launch_tc<BN, EPI_F16_XKV>(pl, d, s); break;
     case EPI_F32: launch_tc<BN, EPI_F32>(pl, d, s); break;
     case EPI_QKV_CACHE: launch_tc<BN, EPI_QKV_CACHE>(pl, d, s); break;
-    case EPI_RESID_ATOMIC: launch_tc<BN, EPI_RESID_ATOMIC>(pl, d, s); break;
     default: throw Error("unknown GEMM epilogue");
   }
 }
 
-static GemmDev make_dev(const GemmArgs& a, int tiles_m, int tiles_n, int num_kb, int ksplit) {
+static GemmDev make_dev(const GemmArgs& a, int tiles_m, int tiles_n, int num_kb) {
   GemmDev d{};
-  d.ksplit = ksplit;
   d.batch = a.a_batch;
   d.tiles_m = tiles_m;
   d.tiles_n = tiles_n;
@@ -371,10 +353,8 @@ static GemmDev make_dev(const GemmArgs& a, int tiles_m, int tiles_n, int num_kb,
 }
 
 void gemm_run(const GemmPlan& pl, cudaStream_t stream) {
-  const GemmDev d = make_dev(pl.a, pl.tiles_m, pl.tiles_n, pl.num_kb, pl.ksplit);
-  if (pl.block_n == 256)
-    dispatch_epi<256>(pl, d, stream);
-  else if (pl.block_n == 128)
+  const GemmDev d = make_dev(pl.a, pl.tiles_m, pl.tiles_n, pl.num_kb);
+  if (pl.block_n == 128)
     dispatch_epi<128>(pl, d, stream);
   else
     dispatch_epi<32>(pl, d, stream);
@@ -422,8 +402,6 @@ __global__ void gemm_ref_kernel(const __half* __restrict__ A, int a_rows, int a_
     }
   } else if (epi == EPI_RESID_F32) {
     reinterpret_cast<float*>(p.out)[idx] = p.resid[idx] + acc;
-  } else if (epi == EPI_RESID_ATOMIC) {
-    reinterpret_cast<float*>(p.out)[idx] += acc;  // one thread per element: a plain in-place add
   } else if (epi == EPI_GELU_POS_F32) {
     reinterpret_cast<float*>(p.out)[idx] = acc + p.pos[(long long)row * p.N + n];
   } else {
@@ -432,7 +410,7 @@ __global__ void gemm_ref_kernel(const __half* __restrict__ A, int a_rows, int a_
 }
 
 void gemm_ref_run(const GemmArgs& a, cudaStream_t stream) {
-  const GemmDev d = make_dev(a, 0, 0, 0, 1);
+  const GemmDev d = make_dev(a, 0, 0, 0);
   dim3 block(32, 8);
   dim3 grid(ceil_div(a.N, 32), ceil_div(a.rows, 8), a.a_batch);
   gemm_ref_kernel<<<grid, block, 0, stream>>>(a.A, a.a_rows, a.a_cols, a.a_row_stride,

@@ -52,7 +52,7 @@ struct Encoded {
 struct Model {
   b2w_config cfg{};
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   int cpad = 128;   // mel channels padded to a multiple of 64
   int vpad = 0;     // vocabulary padded to a multiple of 16
   cudaStream_t stream = nullptr;
@@ -127,7 +127,7 @@ struct Model {
   // de-quantised values (B2W_W8_FAKE=1: the reference the int8 stream is tested against).
   bool w8 = false, w8_fake = false;
   bool use_dstep = true;
-  // many-row persistent step kernel (bstep.cu): decoder weights as 16 KB UMMA atoms + per-row sums for the deferred LayerNorm
+  // many-row persistent step kernel (bstep.cu): decoder weights as 16 KB wgmma atoms + per-row sums for the deferred LayerNorm
   bool use_bstep = true;     // B2W_BSTEP=0 falls back to the multi-kernel step for R > 8
   bool bstep_all = false;    // B2W_BSTEP=all: also for R <= 8 (instead of dstep_kernel)
   int bstep_stop = 0;        // B2W_BSTEP_STOP=n: run only the first n grid phases of every step (debug)
@@ -135,7 +135,7 @@ struct Model {
   BLayer* d_blayers = nullptr;
   const void* logit_atoms = nullptr;
   const float* logit_scale = nullptr;
-  float *d_qkv32 = nullptr, *d_cq32 = nullptr, *d_h32 = nullptr, *d_stats = nullptr;
+  float *d_qkv32 = nullptr, *d_cq32 = nullptr, *d_h32 = nullptr, *d_stats = nullptr, *d_gpart = nullptr, *d_stpart = nullptr;
   __half *d_h16 = nullptr, *d_xn16 = nullptr;
   bool use_mma_xattn = true;  // decode cross attention on mma.sync (dstep.cu) instead of the SIMT kernel (B2W_XATTN_IMPL=simt)
   DecBindings h_bind{};

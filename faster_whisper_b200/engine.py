@@ -3,7 +3,7 @@ faster-whisper consumes (reference ``faster_whisper/transcribe.py:13,689-698,209
 1446-1459,1709-1715,1823,1875``; SURVEY.md §8b): ``Whisper``, ``StorageView``, ``WhisperGenerationResult``.
 
 There is no CPU path and no fallback: importing works anywhere (so host logic can be tested), but creating a
-model, computing a log-mel or encoding raises ``RuntimeError`` unless the CUDA library loads and a B200 is present.
+model, computing a log-mel or encoding raises ``RuntimeError`` unless the CUDA library loads and an H100 (sm_90) is present.
 """
 
 from __future__ import annotations
@@ -294,7 +294,7 @@ class Whisper:
         if device not in ("auto", "cuda", "cpu"):
             raise ValueError(f"unsupported device {device}")
         if device == "cpu":
-            raise ValueError("This engine is B200-only: device='cpu' is not available (no CPU fallback by design)")
+            raise ValueError("This engine is H100-only: device='cpu' is not available (no CPU fallback by design)")
         if compute_type not in _COMPUTE_TYPES:
             raise ValueError(f"Invalid compute type: {compute_type}")
         lib = load_library()

@@ -3,7 +3,7 @@
 Mirrors ``faster_whisper/feature_extractor.py:4-230`` (constructor arguments, attributes, ``__call__``
 semantics including the ``chunk_length`` side effect at ``:203-205``).  ``__call__`` hands the waveform to the
 fused CUDA kernel through the C ABI (``b2w_logmel``); there is no NumPy fallback — without the CUDA library
-and a B200 the call raises.
+and an H100 the call raises.
 """
 
 from __future__ import annotations

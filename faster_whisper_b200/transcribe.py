@@ -1,4 +1,4 @@
-"""``WhisperModel`` and ``BatchedInferencePipeline`` with faster-whisper's public surface, driving the B200 engine.
+"""``WhisperModel`` and ``BatchedInferencePipeline`` with faster-whisper's public surface, driving the H100 engine.
 
 Interface mirrored from ``faster_whisper/transcribe.py`` (reference tree): result/option dataclasses ``:31-108``,
 ``BatchedInferencePipeline`` ``:111-617``, ``WhisperModel`` ``:620-1841`` and the helper functions ``:1844-1941``.

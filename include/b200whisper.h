@@ -1,5 +1,5 @@
 /*
- * libb200whisper — C ABI of the B200-native Whisper engine.
+ * libb200whisper — C ABI of the H100-native Whisper engine.
  *
  * This is the drop-in boundary for the hot path of SYSTRAN/faster-whisper: every entry point replaces one
  * member of the `ctranslate2` Python API exactly as `faster_whisper/transcribe.py` consumes it (file:line
@@ -160,10 +160,10 @@ int b2w_span_end(b2w_model* m, double* ms_out);
 int b2w_counters_get(b2w_model* m, int64_t* launches, int64_t* decode_steps, double* decode_alg_bytes);
 
 /* ---- test hooks (used by tests/ only) ----------------------------------------------------------- */
-/* C = epilogue(A[M,K] * W[N,K]^T + bias) through the tcgen05 (impl=0) or reference SIMT (impl=1) GEMM. */
+/* C = epilogue(A[M,K] * W[N,K]^T + bias) through the wgmma (impl=0) or reference SIMT (impl=1) GEMM. */
 int b2w_debug_gemm(int32_t device, int32_t impl, const float* a, const float* w, const float* bias,
                    int32_t M, int32_t N, int32_t K, int32_t gelu, float* c_out);
-/* softmax(QK^T/8)V for [B,T,H*64] fp16-rounded inputs through the tcgen05 (0) or reference (1) kernel. */
+/* softmax(QK^T/8)V for [B,T,H*64] fp16-rounded inputs through the wgmma (0) or reference (1) kernel. */
 int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t B, int32_t T, int32_t H,
                         float* out);
 /* one decode-style skinny GEMM y[R,N] = x[R,K] W[N,K]^T + b through the mma.sync (0) or reference (1) path */

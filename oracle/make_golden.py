@@ -1,6 +1,6 @@
-"""Generates tests/golden/*.npz|json by RUNNING THE REFERENCE (imported from /root/reference with stubs).
+"""Generates tests/golden/*.npz|json by RUNNING THE REFERENCE (imported from the reference tree with stubs, oracle/refload.py).
 
-TEST INFRASTRUCTURE ONLY.  Run in the build container (the GPU box has no /root/reference):
+TEST INFRASTRUCTURE ONLY.  Run where the reference tree exists ($B2W_REFERENCE_ROOT):
 
     python oracle/make_golden.py
 
@@ -20,7 +20,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from faster_whisper_b200.synthetic import make_tokenizer, synthetic_audio  # noqa: E402
-from oracle.refload import load_reference  # noqa: E402
+from oracle.refload import REFERENCE_ROOT, load_reference  # noqa: E402
 
 
 def read_wav(path, seconds):
@@ -31,13 +31,15 @@ def read_wav(path, seconds):
 
 
 def main():
+    if not REFERENCE_ROOT:
+        raise SystemExit("make_golden.py runs the reference: set B2W_REFERENCE_ROOT to the faster-whisper source tree")
     fw = load_reference()
     out = {}
     for nm in (80, 128):
         fe = fw.feature_extractor.FeatureExtractor(feature_size=nm)
         for n in (0, 159, 160, 4000, 48000):
             out[f"synth_{nm}_{n}"] = fe(synthetic_audio(5, n / 16000.0))
-    speech = read_wav("/root/reference/tests/data/physicsworks.wav", 30.0)
+    speech = read_wav(os.path.join(REFERENCE_ROOT, "tests", "data", "physicsworks.wav"), 30.0)
     out["speech_pcm_head"] = speech[:48000]
     for nm in (80, 128):
         fe = fw.feature_extractor.FeatureExtractor(feature_size=nm)

@@ -1,22 +1,25 @@
-"""Import the UNMODIFIED reference package from /root/reference with its absent native deps stubbed.
+"""Import the UNMODIFIED reference package from a faster-whisper source tree with its absent native deps stubbed.
 
 TEST INFRASTRUCTURE ONLY (see oracle/whisper_oracle.py).  ``av``, ``ctranslate2`` and ``onnxruntime`` are
 not installed in this image (SURVEY.md §8c); the reference's pure-Python host layer imports fine once
 empty modules of those names exist.  ``ctranslate2`` can instead be bound to a shim backed by an engine
 (``oracle/ct2_shim.py``) so the reference's own ``transcribe.py`` drives our engine or the oracle.
-Nothing here may be used on the GPU box: /root/reference does not exist there.
+The tree is looked for at $B2W_REFERENCE_ROOT.  Tests do not need it: what they compare against is
+stored under tests/golden/ (``RecordedReference``, gzip-compressed JSON); with the tree present and B2W_RECORD_REFERENCE=1 it is recorded again.
 """
+import gzip
 import importlib
 import importlib.machinery
+import json
 import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("B2W_REFERENCE_ROOT", "")
 
 
 def reference_available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "faster_whisper"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "faster_whisper"))
 
 
 def load_reference(ct2_module=None):
@@ -46,3 +49,31 @@ def load_reference(ct2_module=None):
         return importlib.import_module("faster_whisper")
     finally:
         sys.path.remove(REFERENCE_ROOT)
+
+
+def canon(x):
+    """The JSON form of a value (tuples -> lists, NumPy scalars -> Python numbers)."""
+    return json.loads(json.dumps(x, default=lambda o: o.item() if hasattr(o, "item") else o.tolist()))
+
+
+class RecordedReference:
+    """Values computed by the reference, stored as gzip-compressed JSON: ``get(key, fn)`` runs ``fn`` (on the reference) and stores
+    its result when recording (B2W_RECORD_REFERENCE=1, reference tree at $B2W_REFERENCE_ROOT), and reads the stored result otherwise."""
+
+    def __init__(self, path: str):
+        self.path = path
+        self.record = os.environ.get("B2W_RECORD_REFERENCE") == "1"
+        if self.record and not reference_available():
+            raise RuntimeError("B2W_RECORD_REFERENCE=1 needs the reference tree at $B2W_REFERENCE_ROOT")
+        self.store = {}
+        if os.path.exists(path):
+            with gzip.open(path, "rt") as f:
+                self.store = json.load(f)
+
+    def get(self, key, fn):
+        if self.record:
+            self.store[key] = canon(fn())
+            data = json.dumps(self.store, sort_keys=True, separators=(",", ":")).encode()
+            with open(self.path, "wb") as f, gzip.GzipFile(fileobj=f, mode="wb", mtime=0) as z:  # mtime 0: same bytes for the same values
+                z.write(data)
+        return self.store[key]

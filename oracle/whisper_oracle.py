@@ -4,14 +4,14 @@
 ``cpu_baseline`` / ``--impl reference`` legs may import this file, and only as the checker or the timed
 CPU baseline.  The product (``faster_whisper_b200``) never imports it and has no CPU fallback.
 
-What is restated, and from where (paths relative to ``/root/reference``):
+What is restated, and from where (paths relative to the reference tree):
 
 * ``mel_filters`` / ``log_mel``      <- ``faster_whisper/feature_extractor.py:24-65`` and ``:198-230``
   (**pinned**: checked bit-for-tolerance against the reference class itself, see
   ``oracle/make_golden.py`` and ``tests/test_oracle.py``).
 * ``WhisperOracle.encode`` / decoder  <- the OpenAI Whisper architecture that ``ctranslate2.models.Whisper``
   executes (call sites ``faster_whisper/transcribe.py:209,1400``).  CTranslate2 (``ctranslate2>=4.0,<5``,
-  ``requirements.txt:1``) is a pip dependency that is *not* vendored under ``/root/reference`` and is not
+  ``requirements.txt:1``) is a pip dependency that is *not* vendored in the reference tree and is not
   installed here, so the network math is cross-checked against ``transformers.WhisperForConditionalGeneration``
   with shared weights (``oracle/check_against_transformers.py``) — a check of our restatement, not of CT2.
 * ``WhisperOracle.generate``          <- CTranslate2 4.x ``Whisper.generate`` semantics as consumed at

@@ -84,7 +84,7 @@ def test_batched_decode_multilingual_geometry(micro_ml):
 
 @pytest.mark.parametrize("n_chunks,beam", [(1, 5), (3, 1), (1, 1)])
 def test_many_row_kernel_on_few_rows(micro_ml, n_chunks, beam):
-    """B2W_BSTEP=all routes R <= 8 through the many-row kernel too (UMMA N = 16): same tokens as the oracle."""
+    """B2W_BSTEP=all routes R <= 8 through the many-row kernel too (wgmma N = 16): same tokens as the oracle."""
     st = micro_ml["tokens"]
     eng = make_engine(micro_ml, B2W_BSTEP="all")
     feats = features_for(micro_ml, n_chunks, seed=310)
@@ -137,3 +137,23 @@ def test_many_row_kernel_other_beam_shapes(micro, n_chunks, beam, extra):
     prompts = [[st.sot_prev, 900, 901, st.sot]] * n_chunks  # timestamps on
     exact, n = compare(eng, micro, feats, prompts, beam_size=beam, max_length=40, repetition_penalty=1.2, no_repeat_ngram_size=3, **extra)
     assert 2 * exact >= n, (exact, n)
+
+
+def test_repeated_batched_steps_are_bit_identical(micro_ml):
+    """16 chunks x beam 5 = 80 rows through the many-row kernel, twice on the same inputs.  The split-K sums, the LayerNorm statistics
+    and the prefill's residual GEMMs are reduced in a fixed order, so tokens, scores and the last step's residual stream, statistics and
+    logits are the same bits every run (fp32 atomics let near-tied beams flip between runs of the benchmark)."""
+    st, dims = micro_ml["tokens"], micro_ml["dims"]
+    eng = make_engine(micro_ml)
+    feats = features_for(micro_ml, 16, seed=60)
+    prompts = [[st.sot, st.lang_begin, st.transcribe, st.no_timestamps]] * 16
+    R, L = 16 * 5, dims.n_text_layer
+    runs = []
+    for _ in range(2):
+        res = eng.generate(eng.encode(feats), prompts, beam_size=5, max_length=40, suppress_tokens=[st.eot], return_scores=True)
+        bufs = [eng.debug_fetch(which, n) for which, n in ((0, R * dims.n_text_state), (7, 3 * L * R * 2), (8, R * dims.n_vocab))]
+        runs.append(([r.sequences_ids[0] for r in res], [r.scores[0] for r in res], bufs))
+    (t0, s0, b0), (t1, s1, b1) = runs
+    assert t0 == t1 and s0 == s1
+    for name, x, y in zip(("residual stream", "LayerNorm statistics", "logits"), b0, b1):
+        assert np.array_equal(x, y), (name, np.abs(x - y).max())

@@ -58,7 +58,7 @@ def test_logmel_silence_and_impulse():
     assert np.abs(got - want).max() < 2e-3
 
 
-# ---- dense GEMM (tcgen05) -----------------------------------------------------------------------------
+# ---- dense GEMM (wgmma) -------------------------------------------------------------------------------
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("shape", [(128, 128, 64), (300, 384, 128), (1500, 1280, 1280), (3001, 256, 192), (257, 5120, 320)])
 def test_gemm_vs_numpy(impl, shape):
@@ -81,7 +81,7 @@ def test_gemm_gelu_epilogue():
     assert np.abs(got - want).max() < 4e-3
 
 
-# ---- encoder attention (tcgen05 flash) -------------------------------------------------------------------
+# ---- encoder attention (wgmma flash) ---------------------------------------------------------------------
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("T", [1500, 128, 77])
 def test_attention_vs_numpy(impl, T):

@@ -12,6 +12,12 @@ from faster_whisper_b200 import utils, vad
 from faster_whisper_b200.config import MODEL_DIMS, special_tokens
 from faster_whisper_b200.synthetic import make_tokenizer
 from faster_whisper_b200.tokenizer import Tokenizer
+from oracle.refload import RecordedReference, canon
+
+
+def recorded_reference():
+    """What the reference returned for the comparisons below (tests/golden/reference_golden.json.gz, recorded by oracle/refload.py)."""
+    return RecordedReference(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_golden.json.gz"))
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -104,21 +110,21 @@ def test_transcribe_signatures():
     seq = inspect.signature(T.WhisperModel.transcribe).parameters
     bat = inspect.signature(T.BatchedInferencePipeline.transcribe).parameters
     assert set(bat) - set(seq) == {"batch_size"} and not set(seq) - set(bat)
-    from oracle.refload import load_reference, reference_available
+    from oracle.refload import load_reference
 
-    if reference_available():
-        R = load_reference().transcribe
-        for ours, theirs in ((T.WhisperModel.transcribe, R.WhisperModel.transcribe),
-                             (T.BatchedInferencePipeline.transcribe, R.BatchedInferencePipeline.transcribe),
-                             (T.WhisperModel.__init__, R.WhisperModel.__init__),
-                             (T.WhisperModel.detect_language, R.WhisperModel.detect_language),
-                             (T.WhisperModel.get_prompt, R.WhisperModel.get_prompt)):
-            a, b = inspect.signature(ours).parameters, inspect.signature(theirs).parameters
-            assert list(a) == list(b), (ours.__qualname__, list(a), list(b))
-            for k in a:
-                assert a[k].default == b[k].default, (ours.__qualname__, k)
-        for cls in ("Word", "Segment", "TranscriptionOptions", "TranscriptionInfo"):
-            assert [f for f in getattr(T, cls).__dataclass_fields__] == [f for f in getattr(R, cls).__dataclass_fields__]
+    rec = recorded_reference()
+    R = load_reference().transcribe if rec.record else None
+
+    def signature(fn):  # parameter names and the repr of their defaults
+        return [[k, repr(v.default)] for k, v in inspect.signature(fn).parameters.items()]
+
+    for name in ("WhisperModel.transcribe", "BatchedInferencePipeline.transcribe", "WhisperModel.__init__", "WhisperModel.detect_language",
+                 "WhisperModel.get_prompt"):
+        cls, meth = name.split(".")
+        want = rec.get("signature/" + name, lambda: signature(getattr(getattr(R, cls), meth)))
+        assert canon(signature(getattr(getattr(T, cls), meth))) == want, name
+    for cls in ("Word", "Segment", "TranscriptionOptions", "TranscriptionInfo"):
+        assert [f for f in getattr(T, cls).__dataclass_fields__] == rec.get("fields/" + cls, lambda: list(getattr(R, cls).__dataclass_fields__))
 
 
 def test_tokenizer_wrapper(tok):
@@ -214,7 +220,6 @@ def test_unloaded_model_is_never_dereferenced():
         E._lib = old_lib
 
 
-@pytest.mark.skipif(not __import__("oracle.refload", fromlist=["reference_available"]).reference_available(), reason="reference tree not mounted (build container only)")
 def test_tokenizer_matches_the_reference_class_on_random_sequences():
     """Our Tokenizer wrapper against the reference's own class (faster_whisper/tokenizer.py, imported unmodified) over the same HF tokenizer:
     sot sequence, non-speech set, decode, decode_with_timestamps and the word splitting (space-based languages and the unicode path of
@@ -223,25 +228,29 @@ def test_tokenizer_matches_the_reference_class_on_random_sequences():
 
     from oracle.refload import load_reference
 
-    fw = load_reference()
-    ref_cls = sys.modules[fw.__name__ + ".tokenizer"].Tokenizer
+    rec = recorded_reference()
+    ref_cls = sys.modules[load_reference().__name__ + ".tokenizer"].Tokenizer if rec.record else None
     hf = make_tokenizer(51866)
     rng = np.random.default_rng(0)
+
+    def specials(t):
+        return [t.sot_sequence, t.non_speech_tokens, [t.transcribe, t.translate, t.sot, t.sot_lm, t.sot_prev, t.eot, t.no_timestamps, t.no_speech,
+                                                      t.timestamp_begin]]
+
+    def outputs(t, ids, ts):
+        return [t.split_to_word_tokens(ids), t.decode_with_timestamps(ts), t.decode(ids), t.encode(" hello wor")]
+
     for lang in ["en", "zh", "ja", "th", "de", "yue"]:
-        ours, ref = Tokenizer(hf, True, task="transcribe", language=lang), ref_cls(hf, True, task="transcribe", language=lang)
-        assert ours.sot_sequence == ref.sot_sequence and ours.non_speech_tokens == ref.non_speech_tokens
-        assert (ours.transcribe, ours.translate, ours.sot, ours.sot_lm, ours.sot_prev, ours.eot, ours.no_timestamps, ours.no_speech, ours.timestamp_begin) == (
-            ref.transcribe, ref.translate, ref.sot, ref.sot_lm, ref.sot_prev, ref.eot, ref.no_timestamps, ref.no_speech, ref.timestamp_begin)
+        ours = Tokenizer(hf, True, task="transcribe", language=lang)
+        ref = ref_cls(hf, True, task="transcribe", language=lang) if rec.record else None
+        assert canon(specials(ours)) == rec.get(f"tokenizer/{lang}/specials", lambda: specials(ref))
         for trial in range(120):
             n = int(rng.integers(1, 24))
             ids = [int(x) for x in rng.integers(0, ours.eot, size=n)] + ([ours.eot] if trial % 3 == 0 else [])
-            assert ours.split_to_word_tokens(ids) == ref.split_to_word_tokens(ids), (lang, ids)
             ts = [ours.timestamp_begin + 3] + ids[: n // 2] + [ours.timestamp_begin + 40] * 2 + ids[n // 2:] + [ours.timestamp_begin + 90]
-            assert ours.decode_with_timestamps(ts) == ref.decode_with_timestamps(ts)
-            assert ours.decode(ids) == ref.decode(ids) and ours.encode(" hello wor") == ref.encode(" hello wor")
+            assert canon(outputs(ours, ids, ts)) == rec.get(f"tokenizer/{lang}/{trial}", lambda: outputs(ref, ids, ts)), (lang, ids)
 
 
-@pytest.mark.skipif(not __import__("oracle.refload", fromlist=["reference_available"]).reference_available(), reason="reference tree not mounted (build container only)")
 def test_model_names_and_hub_repositories_match_the_reference():
     """available_models() and the size -> hub repository table are the reference's (utils.py:12-47), entry for entry and in order."""
     import sys
@@ -249,9 +258,10 @@ def test_model_names_and_hub_repositories_match_the_reference():
     from faster_whisper_b200 import utils as ours
     from oracle.refload import load_reference
 
-    fw = load_reference()
-    ref = sys.modules[fw.__name__ + ".utils"]
-    assert ours.available_models() == ref.available_models()
-    assert ours._HUB_REPOS == ref._MODELS
-    assert ours.format_timestamp(3723.456, always_include_hours=True, decimal_marker=",") == ref.format_timestamp(3723.456, always_include_hours=True, decimal_marker=",")
-    assert ours.format_timestamp(59.999) == ref.format_timestamp(59.999)
+    rec = recorded_reference()
+    ref = sys.modules[load_reference().__name__ + ".utils"] if rec.record else None
+    assert ours.available_models() == rec.get("utils/available_models", lambda: ref.available_models())
+    assert list(ours._HUB_REPOS.items()) == [tuple(kv) for kv in rec.get("utils/models", lambda: list(ref._MODELS.items()))]
+    assert ours.format_timestamp(3723.456, always_include_hours=True, decimal_marker=",") == rec.get(
+        "utils/format_timestamp_hours", lambda: ref.format_timestamp(3723.456, always_include_hours=True, decimal_marker=","))
+    assert ours.format_timestamp(59.999) == rec.get("utils/format_timestamp", lambda: ref.format_timestamp(59.999))

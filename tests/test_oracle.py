@@ -1,5 +1,6 @@
-"""CPU: the oracle against the reference's own outputs (golden fixtures made by oracle/make_golden.py, and the
-reference itself when /root/reference is mounted), plus internal consistency of its search code."""
+"""CPU: the oracle against the reference's own outputs (golden fixtures made by oracle/make_golden.py and recorded through
+oracle/refload.py), plus internal consistency of its search code."""
+import hashlib
 import os
 
 import numpy as np
@@ -8,7 +9,6 @@ import pytest
 from conftest import fake_logits_numpy
 from faster_whisper_b200.synthetic import synthetic_audio
 from oracle import whisper_oracle as orc
-from oracle.refload import reference_available
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -30,17 +30,27 @@ def test_log_mel_matches_reference_goldens(mel_gold, n_mels):
     assert np.abs(got - mel_gold[f"speech_head_{n_mels}"]).max() <= 1e-6
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not mounted")
-def test_log_mel_matches_reference_live():
-    from oracle.refload import load_reference
+def _digest(a):
+    a = np.ascontiguousarray(a)
+    return [str(a.dtype), list(a.shape), hashlib.sha256(a.tobytes()).hexdigest()]
 
-    fw = load_reference()
+
+def test_log_mel_matches_reference_live():
+    """The reference's FeatureExtractor (mel filters and log-mel of four clip lengths) against the oracle, bit for bit: dtype, shape
+    and SHA-256 of the reference's arrays are stored in tests/golden/reference_golden.json.gz (oracle/refload.py records them).  The
+    digests pin the NumPy the goldens were recorded with (stored beside them): under another NumPy a changed FFT or rounding shows
+    here even if the oracle is still right — re-record against the reference tree then."""
+    from oracle.refload import RecordedReference, load_reference
+
+    rec = RecordedReference(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_golden.json.gz"))
+    fw = load_reference() if rec.record else None
+    note = "goldens recorded under NumPy %s, running %s" % (rec.get("log_mel/numpy_version", lambda: np.__version__), np.__version__)
     for nm in (80, 128):
-        fe = fw.feature_extractor.FeatureExtractor(feature_size=nm)
-        assert np.array_equal(fe.mel_filters, orc.mel_filters(n_mels=nm))
+        fe = fw.feature_extractor.FeatureExtractor(feature_size=nm) if fw else None
+        assert _digest(orc.mel_filters(n_mels=nm)) == rec.get(f"log_mel/filters_{nm}", lambda: _digest(fe.mel_filters)), note
         for n in (1, 161, 30000, 480000):
             x = synthetic_audio(9, n / 16000.0)
-            assert np.array_equal(fe(x), orc.log_mel(x, nm))
+            assert _digest(orc.log_mel(x, nm)) == rec.get(f"log_mel/{nm}_{n}", lambda: _digest(fe(x))), note
 
 
 def test_pad_or_trim():

@@ -1,4 +1,4 @@
-// Floor of one dependent "phase" on B200: all CTAs publish a little data, grid barrier, all CTAs read what the others wrote.
+// Floor of one dependent "phase" on the GPU: all CTAs publish a little data, grid barrier, all CTAs read what the others wrote.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -62,15 +62,15 @@ __global__ void phase_floor(float* data, unsigned* bar, int iters, int mode, lon
 int main() {
   float* data; unsigned* bar; long long* out;
   CK(cudaMalloc(&data, 1 << 20)); CK(cudaMemset(data, 0, 1 << 20));
-  CK(cudaMalloc(&bar, 4)); CK(cudaMalloc(&out, 148 * 3 * 8));
-  for (int grid : {148, 74, 16}) {
+  CK(cudaMalloc(&bar, 4)); CK(cudaMalloc(&out, 132 * 3 * 8));
+  for (int grid : {132, 66, 16}) {
     for (int mode = 0; mode < 4; ++mode) {
       CK(cudaMemset(bar, 0, 4));
       int iters = 2000;
       void* args[] = {&data, &bar, &iters, &mode, &out};
       CK(cudaLaunchCooperativeKernel((void*)phase_floor, dim3(grid), dim3(256), args, 0, 0));
       CK(cudaDeviceSynchronize());
-      std::vector<long long> h(148 * 3);
+      std::vector<long long> h(132 * 3);
       CK(cudaMemcpy(h.data(), out, grid * 3 * 8, cudaMemcpyDeviceToHost));
       double b = 0, r = 0, e = 0;
       for (int i = 0; i < grid; ++i) { b += h[i * 3]; r += h[i * 3 + 1]; e += h[i * 3 + 2]; }

@@ -1,5 +1,5 @@
 // Latency of one "weight tile" fetch (40 KB contiguous per CTA, 10 x 16-byte loads per thread in flight) as a function of
-// the footprint the tiles are drawn from: separates TLB-reach effects from L2/HBM effects on B200.
+// the footprint the tiles are drawn from: separates TLB-reach effects from L2/HBM effects on the GPU.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -46,7 +46,7 @@ int main() {
   CK(cudaMemset(buf, 1, cap));
   long long* d_cycles;
   unsigned* d_sink;
-  CK(cudaMalloc(&d_cycles, 148 * sizeof(long long)));
+  CK(cudaMalloc(&d_cycles, 132 * sizeof(long long)));
   CK(cudaMalloc(&d_sink, 4));
   struct Case { const char* name; size_t footprint, step; };
   Case cases[] = {
@@ -58,14 +58,14 @@ int main() {
   };
   for (auto& c : cases) {
     for (int rep = 0; rep < 2; ++rep) {
-      tile_latency<<<148, 256>>>(buf, c.footprint, c.step, 2000, d_cycles, d_sink);
+      tile_latency<<<132, 256>>>(buf, c.footprint, c.step, 2000, d_cycles, d_sink);
       CK(cudaDeviceSynchronize());
     }
-    std::vector<long long> h(148);
-    CK(cudaMemcpy(h.data(), d_cycles, 148 * sizeof(long long), cudaMemcpyDeviceToHost));
+    std::vector<long long> h(132);
+    CK(cudaMemcpy(h.data(), d_cycles, 132 * sizeof(long long), cudaMemcpyDeviceToHost));
     long long mn = 1ll << 60, mx = 0, sum = 0;
     for (auto v : h) { mn = v < mn ? v : mn; mx = v > mx ? v : mx; sum += v; }
-    printf("%-58s  cycles/tile: mean %lld  min %lld  max %lld\n", c.name, sum / 148, mn, mx);
+    printf("%-58s  cycles/tile: mean %lld  min %lld  max %lld\n", c.name, sum / 132, mn, mx);
   }
   return 0;
 }

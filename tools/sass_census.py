@@ -1,8 +1,7 @@
-"""Per-kernel SASS instruction census of libb200whisper.so (cuobjdump -sass): which kernels are tcgen05 (UTC*MMA, LDTM/STTM,
-UTCBAR), which use TMA (UTMALDG tensor loads, UBLKCP bulk copies, UBLKRED bulk reductions) and which are mma.sync (HMMA).
-Writes a table to stdout; commit it under profiles/ so the "hand-written tcgen05/TMA" claims are checkable without a GPU.
+"""Per-kernel SASS instruction census of libb200whisper.so (cuobjdump -sass): which kernels are wgmma (HGMMA), which use TMA
+(UTMALDG tensor loads, UBLKCP bulk copies, UBLKRED bulk reductions) and which are mma.sync (HMMA).  Needs no GPU.
 
-    python tools/sass_census.py > profiles/r2_sass_census.txt
+    python tools/sass_census.py
 """
 import os
 import re
@@ -13,8 +12,7 @@ from collections import Counter, OrderedDict
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "faster_whisper_b200", "libb200whisper.so")
 PATTERNS = OrderedDict([
-    ("UTCHMMA/UTCQMMA (tcgen05.mma)", r"\bUTC[HQ]MMA"), ("LDTM (tcgen05.ld)", r"\bLDTM"), ("STTM (tcgen05.st)", r"\bSTTM"),
-    ("UTCBAR (tcgen05.commit)", r"\bUTCBAR"), ("UTMALDG (TMA tensor load)", r"\bUTMALDG"), ("UBLKCP (TMA bulk copy)", r"\bUBLKCP"),
+    ("HGMMA (wgmma)", r"\bHGMMA"), ("UTMALDG (TMA tensor load)", r"\bUTMALDG"), ("UBLKCP (TMA bulk copy)", r"\bUBLKCP"),
     ("UBLKRED (TMA bulk reduce)", r"\bUBLKRED"), ("SYNCS (mbarrier)", r"\bSYNCS"), ("HMMA (mma.sync)", r"\bHMMA"), ("LDGSTS (cp.async)", r"\bLDGSTS"),
     ("RED/ATOM global", r"\b(RED|ATOMG|ATOM)\b"), ("total instructions", r"^\s+/\*[0-9a-f]{4,}\*/"),
 ])
@@ -35,7 +33,7 @@ def main():
             if re.search(pat, line):
                 kernels[cur][name] += 1
     demangle = subprocess.run(["c++filt"], input="\n".join(kernels), capture_output=True, text=True).stdout.splitlines()
-    print("SASS census of faster_whisper_b200/libb200whisper.so (sm_100a), one row per kernel; counts are static instruction counts\n")
+    print("SASS census of faster_whisper_b200/libb200whisper.so (sm_90a), one row per kernel; counts are static instruction counts\n")
     cols = list(PATTERNS)
     print("%-70s " % "kernel" + " ".join("%9s" % c.split(" ")[0][:9] for c in cols))
     for (mangled, cnt), name in zip(kernels.items(), demangle):
