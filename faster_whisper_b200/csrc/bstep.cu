@@ -33,6 +33,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "bstep.h"
 #include "common.cuh"
@@ -1417,6 +1418,50 @@ void bstep_launch(const BStepArgs& a, int grid, cudaStream_t s) {
   void* args[] = {&copy};
   B2W_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(bstep_kernel), dim3(grid), dim3(kBsLaunch), args, smem, s));
   count_launch();
+}
+
+// Stamps of the last step ([0] = start, then (arrive, release) of every grid barrier, then end) and the cycle counters at
+// prof + 3000, written by bstep_kernel into a.prof; the counters are cleared after printing.
+void bstep_print_profile(const BStepArgs& a, cudaStream_t s) {
+  B2W_CUDA(cudaStreamSynchronize(s));
+  const int L = a.L, nstamps = 1 + 2 * (2 + 9 * L) + 1;
+  std::vector<unsigned long long> t(nstamps);
+  B2W_CUDA(cudaMemcpy(t.data(), a.prof, nstamps * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  static const char* names[9] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1", "gelu", "ffn2"};
+  double work[9] = {0}, wait[9] = {0};
+  unsigned long long prev = t[2];
+  for (int l = 0; l < L; ++l)
+    for (int ph = 0; ph < 9; ++ph) {
+      const int bi = 1 + 2 * (1 + l * 9 + ph);
+      work[ph] += double(t[bi] - prev);
+      wait[ph] += double(t[bi + 1] - t[bi]);
+      prev = t[bi + 1];
+    }
+  const int bf = 1 + 2 * (1 + 9 * L);
+  fprintf(stderr, "[bstep prof] last step (R=%d): total %.1f us; embed %.1f us; final-LN %.1f us; logits %.1f us\n", a.R, (t[nstamps - 1] - t[0]) / 1e3,
+          (t[2] - t[0]) / 1e3, (t[bf] - prev) / 1e3, (t[nstamps - 1] - t[bf + 1]) / 1e3);
+  for (int ph = 0; ph < 9; ++ph)
+    fprintf(stderr, "[bstep prof]   %-10s work %.2f us  barrier wait %.2f us (CTA 0, mean over %d layers)\n", names[ph], work[ph] / L / 1e3,
+            wait[ph] / L / 1e3, L);
+  {
+    std::vector<unsigned long long> f(8 * 16);
+    B2W_CUDA(cudaMemcpy(f.data(), a.prof + 3000, f.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemset(a.prof + 3000, 0, f.size() * sizeof(unsigned long long)));
+    if (f[6 * 16 + 15] > 0)
+      fprintf(stderr, "[bstep prof]   self-attn cycles per 16-key block (CTA 0 warp 0): (unused) %.0f  issue+copy-wait %.0f  compute %.0f; prologue per task total %.0f over %llu blocks\n",
+              (double)f[6 * 16 + 1] / f[6 * 16 + 15], (double)f[6 * 16 + 2] / f[6 * 16 + 15], (double)f[6 * 16 + 3] / f[6 * 16 + 15], (double)f[6 * 16],
+              f[6 * 16 + 15]);
+    if (f[7 * 16 + 15] > 0)
+      fprintf(stderr, "[bstep prof]   cross-attn cycles per tile (CTA 0): tile-wait %.0f  compute %.0f; piece ends total %.0f, prologues total %.0f over %llu tiles\n",
+              (double)f[7 * 16] / f[7 * 16 + 15], (double)f[7 * 16 + 1] / f[7 * 16 + 15], (double)f[7 * 16 + 2], (double)f[7 * 16 + 3], f[7 * 16 + 15]);
+    static const char* kinds[6] = {"qkv", "out", "cross_q", "cross_out", "ffn1", "ffn2"};
+    for (int k = 0; k < 6; ++k) {
+      const double cnt = (double)f[k * 16 + 15];
+      if (cnt > 0)
+        fprintf(stderr, "[bstep prof]   %-9s cycles (CTA 0): stage %.0f  sync %.0f  row statistics %.0f  products + reduction %.0f\n", kinds[k],
+                f[k * 16] / cnt, f[k * 16 + 4] / cnt, f[k * 16 + 5] / cnt, f[k * 16 + 2] / cnt);
+    }
+  }
 }
 
 }  // namespace b2w

@@ -70,5 +70,7 @@ bool bstep_supported(int num_sms, BStepArgs& a);  // fills a.NP / a.u_bytes; fal
 size_t bstep_xpart_floats(const BStepArgs& a);
 void bstep_launch(const BStepArgs& a, int grid, cudaStream_t s);
 int bstep_phase_count(int L);
+// B2W_DSTEP_PROF: prints the per-phase timers of the last step launched with a.prof set (stderr)
+void bstep_print_profile(const BStepArgs& a, cudaStream_t s);
 
 }  // namespace b2w

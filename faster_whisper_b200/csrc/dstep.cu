@@ -29,6 +29,8 @@
 // decode step" of BASELINE.json's north_star.
 #include <math.h>
 
+#include <vector>
+
 #include "common.cuh"
 #include "decode.h"
 #include "dstep.h"
@@ -823,6 +825,43 @@ void dstep_launch(const DStepArgs& a, int grid, cudaStream_t s) {
   void* fn = a.w8 ? reinterpret_cast<void*>(dstep_kernel<true>) : reinterpret_cast<void*>(dstep_kernel<false>);
   B2W_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kDsLaunchThreads), args, smem, s));
   count_launch();
+}
+
+// Stamps of the last step ([0] = start, then (arrive, release) of every barrier, then end) and the cycle counters at prof + 3000,
+// written by dstep_kernel into a.prof; the counters are cleared after printing.
+void dstep_print_profile(const DStepArgs& a, cudaStream_t s) {
+  B2W_CUDA(cudaStreamSynchronize(s));
+  const int L = a.L, nstamps = 1 + 2 * (1 + 8 * L) + 1;
+  std::vector<unsigned long long> t(nstamps);
+  B2W_CUDA(cudaMemcpy(t.data(), a.prof, nstamps * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  // work(p) = arrive_p - release_{p-1}; wait(p) = release_p - arrive_p
+  static const char* names[8] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1", "ffn2"};
+  double work[8] = {0}, wait[8] = {0};
+  unsigned long long prev = t[2];  // release of the embed barrier
+  for (int l = 0; l < L; ++l)
+    for (int ph = 0; ph < 8; ++ph) {
+      const int bi = 1 + 2 * (1 + l * 8 + ph);
+      work[ph] += double(t[bi] - prev);
+      wait[ph] += double(t[bi + 1] - t[bi]);
+      prev = t[bi + 1];
+    }
+  fprintf(stderr, "[dstep prof] last step: total %.1f us; embed %.1f us; logits %.1f us\n", (t[nstamps - 1] - t[0]) / 1e3,
+          (t[2] - t[0]) / 1e3, (t[nstamps - 1] - prev) / 1e3);
+  {
+    std::vector<unsigned long long> f(8 * 16);
+    B2W_CUDA(cudaMemcpy(f.data(), a.prof + 3000, f.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemset(a.prof + 3000, 0, f.size() * sizeof(unsigned long long)));
+    static const char* kinds[7] = {"qkv", "out", "cross_q", "cross_out", "ffn1", "ffn2", "logits"};
+    for (int k = 0; k < 7; ++k) {
+      const double n = (double)f[k * 16 + 15];
+      if (n > 0)
+        fprintf(stderr, "[dstep prof]   %-9s cycles (first item): stage-input %.0f  tile-wait %.0f  mma %.0f  epilogue %.0f\n", kinds[k], f[k * 16] / n,
+                f[k * 16 + 1] / n, f[k * 16 + 2] / n, f[k * 16 + 3] / n);
+    }
+  }
+  for (int ph = 0; ph < 8; ++ph)
+    fprintf(stderr, "[dstep prof]   %-10s work %.2f us  barrier wait %.2f us (CTA 0, mean over %d layers)\n", names[ph], work[ph] / L / 1e3,
+            wait[ph] / L / 1e3, L);
 }
 
 }  // namespace b2w

@@ -61,5 +61,7 @@ size_t dstep_smem_bytes(const DStepArgs& a);
 void dstep_configure();
 int dstep_max_grid(int num_sms, const DStepArgs& a);
 void dstep_launch(const DStepArgs& a, int grid, cudaStream_t s);
+// B2W_DSTEP_PROF: prints the per-phase timers of the last step launched with a.prof set (stderr)
+void dstep_print_profile(const DStepArgs& a, cudaStream_t s);
 
 }  // namespace b2w

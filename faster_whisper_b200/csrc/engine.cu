@@ -60,13 +60,22 @@ static T* dalloc(size_t n) {
   return reinterpret_cast<T*>(p);
 }
 
+// device memory allocated once per model: freed by ~Model through `allocs`
+template <typename T>
+static T* model_alloc(Model* m, size_t n) {
+  T* p = dalloc<T>(n);
+  m->allocs.push_back(p);
+  return p;
+}
+
 Model::~Model() {
   cudaSetDevice(device);
   if (stream) cudaStreamSynchronize(stream);
   for (void* p : allocs) cudaFree(p);
   for (auto& it : pool) cudaFree(it.second);
-  void* ws[] = {e_feats, e_x0, e_x1, e_x, e_xn, e_qkv, e_ao, e_h, e_pcm, e_chunks, e_chunk_max, kcache, vcache, d_x, d_xn,
-                d_q, d_ao, d_h, d_logits, d_xpart, d_counters, d_suppress, sb_blob, d_bind, d_layers, d_bar, d_gpart, d_stpart};
+  // the buffers that are reallocated when a larger shape arrives
+  void* ws[] = {e_feats, e_x0, e_x1, e_x, e_xn, e_qkv, e_ao, e_h, e_pcm, e_chunks, e_chunk_max, kcache, vcache, d_xpart, sb_blob,
+                d_align_heads};
   for (void* p : ws)
     if (p) cudaFree(p);
   if (h_pinned) cudaFreeHost(h_pinned);
@@ -229,8 +238,7 @@ struct Uploader {
   }
   template <typename T>
   T* alloc(size_t n, bool zero = false) {
-    T* p = dalloc<T>(n);
-    m->allocs.push_back(p);
+    T* p = model_alloc<T>(m, n);
     if (zero) B2W_CUDA(cudaMemset(p, 0, n * sizeof(T)));
     return p;
   }
@@ -431,11 +439,11 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
   }
   m->dec_weight_bytes = wbytes;
   m->mel.reset(new MelPlan(cfg.n_mels));
-  m->d_counters = dalloc<int>(64 + 16 * 20 * 64);
+  m->d_counters = model_alloc<int>(m, 64 + 16 * 20 * 64);
   B2W_CUDA(cudaMemset(m->d_counters, 0, (64 + 16 * 20 * 64) * sizeof(int)));
   B2W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->h_pinned), 4096));
-  m->d_suppress = dalloc<uint8_t>(m->vpad);
-  m->d_bind = dalloc<DecBindings>(1);
+  m->d_suppress = model_alloc<uint8_t>(m, m->vpad);
+  m->d_bind = model_alloc<DecBindings>(m, 1);
   decode_configure();
   search_configure();
   gemm_configure();
@@ -446,13 +454,13 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     std::vector<DLayer> hl(L);
     unsigned char* q_scratch = nullptr;
     float* scale_scratch = nullptr;
-    if (m->w8 || m->w8_fake) {
+    if (m->w8) {
       q_scratch = dalloc<unsigned char>((size_t)m->vpad * dt > (size_t)4 * dt * dt ? (size_t)m->vpad * dt : (size_t)4 * dt * dt);
       scale_scratch = dalloc<float>((size_t)std::max(m->vpad, 4 * dt));
     }
     // every decoder matrix is laid out twice: as the <= 8-row kernel's tile stream (dstep.cu) and as the many-row kernel's atom
     // stream (bstep.cu, + row sums for the deferred LayerNorm); with compute_type int8* both streams carry the int8 values
-    const bool want_b = m->use_bstep && dt % 64 == 0 && dt == 64 * cfg.n_text_head;
+    const bool want_b = dt % 64 == 0 && dt == 64 * cfg.n_text_head;
     struct BPack {
       const void* atoms = nullptr;
       const float* scale = nullptr;
@@ -460,11 +468,9 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     };
     auto pack = [&](const __half* W, const float* bias, int N, int K, int ksplit, BPack* bp, bool want_wsum) -> const __half* {
       const __half* tiles = nullptr;
-      if (m->w8 || m->w8_fake) {
+      if (m->w8) {
         // quantise per output channel; W now holds q * scale (what the prefill / multi-kernel paths multiply with)
         dstep_quantize_rows(const_cast<__half*>(W), N, K, q_scratch, scale_scratch, m->stream);
-      }
-      if (m->w8) {
         unsigned char* out8 = up.alloc<unsigned char>(dstep_packed_bytes_i8(N, K, ksplit));
         dstep_pack_tiles_i8(q_scratch, scale_scratch, bias, N, K, ksplit, out8, m->stream);
         tiles = reinterpret_cast<const __half*>(out8);
@@ -518,22 +524,26 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     }
     BPack lp;
     if (packable) m->logit_tiles = pack(m->logit_w, m->logit_b, m->vpad, dt, 1, &lp, false);
-    else m->use_dstep = false;
     if (q_scratch) {
       B2W_CUDA(cudaStreamSynchronize(m->stream));
       cudaFree(q_scratch);
       cudaFree(scale_scratch);
     }
-    m->d_layers = dalloc<DLayer>(L);
+    m->d_layers = model_alloc<DLayer>(m, L);
     B2W_CUDA(cudaMemcpy(m->d_layers, hl.data(), L * sizeof(DLayer), cudaMemcpyHostToDevice));
+    if (packable) {
+      DStepArgs ds{};  // the grid depends on the model only: width, depth, weight format
+      ds.L = L; ds.d = dt; ds.w8 = m->w8 ? 1 : 0; ds.R = 1; ds.T = 1500;
+      m->dstep_grid = dstep_max_grid(m->num_sms, ds);
+    }
     if (want_b && packable) {
       m->logit_atoms = lp.atoms;
       m->logit_scale = lp.scale;
-      m->d_blayers = dalloc<BLayer>(L);
+      m->d_blayers = model_alloc<BLayer>(m, L);
       B2W_CUDA(cudaMemcpy(m->d_blayers, bl.data(), L * sizeof(BLayer), cudaMemcpyHostToDevice));
       m->bstep_packed = true;
     }
-    m->d_bar = dalloc<unsigned>(kBsBarWords);
+    m->d_bar = model_alloc<unsigned>(m, kBsBarWords);
     B2W_CUDA(cudaMemset(m->d_bar, 0, kBsBarWords * sizeof(unsigned)));
   }
   for (int l = L / 2; l < L; ++l)  // default alignment heads: every head of the last half of the decoder (OpenAI Whisper's default)
@@ -709,20 +719,20 @@ static void ensure_decoder_ws(Model* m, int chunks, int slots) {
   const int dt = m->cfg.n_text_state, L = m->cfg.n_text_layer, n_ctx = m->cfg.n_text_ctx;
   if (!m->d_x) {
     const size_t dt128 = (size_t)ceil_div(dt, 128) * 128;  // the many-row step kernel keeps its fp32 buffers n-block-major (128-channel blocks)
-    m->d_x = dalloc<float>((size_t)kMaxRows * dt128);
-    m->d_xn = dalloc<__half>((size_t)kMaxRows * dt);
-    m->d_q = dalloc<__half>((size_t)kMaxRows * dt);
-    m->d_ao = dalloc<__half>((size_t)kMaxRows * dt);
-    m->d_h = dalloc<__half>((size_t)kMaxRows * 4 * dt);
-    m->d_logits = dalloc<float>((size_t)kMaxRows * m->vpad);
-    m->d_qkv32 = dalloc<float>((size_t)kMaxRows * ceil_div(3 * dt, 128) * 128);
-    m->d_cq32 = dalloc<float>((size_t)kMaxRows * dt128);
-    m->d_h32 = dalloc<float>((size_t)kMaxRows * ceil_div(4 * dt, 128) * 128);
-    m->d_h16 = dalloc<__half>((size_t)kMaxRows * 4 * dt);
-    m->d_xn16 = dalloc<__half>((size_t)kMaxRows * dt);
-    m->d_stats = dalloc<float>((size_t)3 * L * kMaxRows * 2 + 4);
-    m->d_gpart = dalloc<float>((size_t)m->num_sms * kMaxRows * 128);  // the many-row step kernel's per-CTA split-K partial tiles
-    m->d_stpart = dalloc<float>((size_t)(dt / 64) * kMaxRows * 2);
+    m->d_x = model_alloc<float>(m, (size_t)kMaxRows * dt128);
+    m->d_xn = model_alloc<__half>(m, (size_t)kMaxRows * dt);
+    m->d_q = model_alloc<__half>(m, (size_t)kMaxRows * dt);
+    m->d_ao = model_alloc<__half>(m, (size_t)kMaxRows * dt);
+    m->d_h = model_alloc<__half>(m, (size_t)kMaxRows * 4 * dt);
+    m->d_logits = model_alloc<float>(m, (size_t)kMaxRows * m->vpad);
+    m->d_qkv32 = model_alloc<float>(m, (size_t)kMaxRows * ceil_div(3 * dt, 128) * 128);
+    m->d_cq32 = model_alloc<float>(m, (size_t)kMaxRows * dt128);
+    m->d_h32 = model_alloc<float>(m, (size_t)kMaxRows * ceil_div(4 * dt, 128) * 128);
+    m->d_h16 = model_alloc<__half>(m, (size_t)kMaxRows * 4 * dt);
+    m->d_xn16 = model_alloc<__half>(m, (size_t)kMaxRows * dt);
+    m->d_stats = model_alloc<float>(m, (size_t)3 * L * kMaxRows * 2 + 4);
+    m->d_gpart = model_alloc<float>(m, (size_t)m->num_sms * kMaxRows * 128);  // the many-row step kernel's per-CTA split-K partial tiles
+    m->d_stpart = model_alloc<float>(m, (size_t)(dt / 64) * kMaxRows * 2);
     B2W_CUDA(cudaMemset(m->d_xn, 0, (size_t)kMaxRows * dt * 2));
     B2W_CUDA(cudaMemset(m->d_ao, 0, (size_t)kMaxRows * dt * 2));
     B2W_CUDA(cudaMemset(m->d_h, 0, (size_t)kMaxRows * 4 * dt * 2));
@@ -867,11 +877,7 @@ static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
 }
 
 static void gv(Model* m, GvArgs a) {
-  if (m->use_ref_gemv && (a.mode == GV_F32)) {
-    skinny_ref(a.x, a.W, a.bias, a.out_f, a.R, a.N, a.K, m->stream);
-    return;
-  }
-  if (a.R >= kTcMinRows && a.K % 64 == 0 && a.N % 32 == 0 && !m->use_ref_gemv) {
+  if (a.R >= kTcMinRows && a.K % 64 == 0 && a.N % 32 == 0) {
     gemm_run(dec_plan(m, a), m->stream);
     if (a.mode == GV_RESID_LN) layernorm_f32_f16(a.xres, a.ln_g, a.ln_b, a.xn_out, a.R, a.N, m->stream);
     return;
@@ -884,20 +890,36 @@ static void bind_encoded(Model* m, const Encoded* e, int chunk0) {
   B2W_CUDA(cudaMemcpyAsync(m->d_bind, &m->h_bind, sizeof(DecBindings), cudaMemcpyHostToDevice, m->stream));
 }
 
-static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots, int splits, int step_base) {
+// 8 key splits (~188 keys each) for the SIMT cross attention: the V tile fits in shared memory next to the scores and even one
+// chunk fills the SMs
+constexpr int kXSplits = 8;
+static_assert(kXSplits >= kDsXSplits, "the SIMT kernel's partial buffer must also hold the mma.sync task's partials");
+
+// Floats of the cross-attention partial buffer for n_chunks x rows_per_chunk rows.  The SIMT kernel's need (kXSplits splits per
+// query group) covers the kDsXSplits-split mma.sync task of both persistent kernels and of its stand-alone launch.
+static size_t xpart_floats(const Model* m, int n_chunks, int rows_per_chunk) {
+  return cross_attn_partial_floats(n_chunks, m->cfg.n_text_head, rows_per_chunk, kXSplits);
+}
+
+// The partial buffer is grown outside graph capture (which forbids cudaMalloc and synchronisation), before any argument block
+// or graph takes its pointer.
+static void ensure_xpart(Model* m, size_t floats) {
+  if (floats <= m->d_xpart_floats) return;
+  B2W_CUDA(cudaStreamSynchronize(m->stream));
+  if (m->d_xpart) cudaFree(m->d_xpart);
+  m->d_xpart = dalloc<float>(floats);
+  m->d_xpart_floats = floats;
+}
+
+// The layered decoder step: one launch per GEMM / attention.  Needs ensure_xpart(m, xpart_floats(m, n_chunks, rows_per_chunk)).
+static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots) {
   const b2w_config& c = m->cfg;
   const int dt = c.n_text_state, L = c.n_text_layer, H = c.n_text_head, R = n_chunks * rows_per_chunk;
   cudaStream_t s = m->stream;
   const SearchBuffers& sb = m->sb;
   embed_ln(sb.tokens_in, sb.rows, m->tok_emb, m->dec_pos, m->dec[0].ln1_g, m->dec[0].ln1_b, m->d_x, m->d_xn, R, dt, c.n_vocab, s);
   const int qgroups = cross_attn_qgroups(rows_per_chunk);
-  const size_t need_part = cross_attn_partial_floats(n_chunks, H, rows_per_chunk, splits);
-  if (need_part > m->d_xpart_floats) {
-    B2W_CUDA(cudaStreamSynchronize(s));
-    if (m->d_xpart) cudaFree(m->d_xpart);
-    m->d_xpart = dalloc<float>(need_part);
-    m->d_xpart_floats = need_part;
-  }
+  B2W_CHECK(m->d_xpart_floats >= xpart_floats(m, n_chunks, rows_per_chunk), "cross-attention partial buffer");
   B2W_CHECK((size_t)n_chunks * H * qgroups <= 16 * 20 * 64, "cross-attention group counters");
   for (int l = 0; l < L; ++l) {
     const DecLayerW& W = m->dec[l];
@@ -907,8 +929,7 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     a.x = m->d_xn; a.W = W.wqkv; a.bias = W.bqkv; a.R = R; a.N = 3 * dt; a.K = dt; a.mode = GV_QKV;
     a.rows = sb.rows; a.kcache = kc; a.vcache = vc; a.d = dt; a.n_ctx = c.n_text_ctx; a.slots = slots; a.out_h = m->d_q;
     gv(m, a);
-    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots,
-                    (long long)n_chunks * slots * c.n_text_ctx, step_base};
+    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots, (long long)n_chunks * slots * c.n_text_ctx, 0};
     dec_self_attn(sa, R, H, s);
     GvArgs o;
     o.x = m->d_ao; o.W = W.wo; o.bias = W.bo; o.R = R; o.N = dt; o.K = dt; o.mode = GV_RESID_LN;
@@ -920,18 +941,18 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     if (m->align_out)
       align_probs(m->d_q, m->d_bind, l, m->d_align_heads, (int)m->align_heads.size(), m->align_out, m->align_n_tok, m->align_nf,
                   m->align_pos0, R, H, 1500, dt, s);
-    if (m->use_mma_xattn && splits >= kDsXSplits && dstep_cross_attn_supported(1500, rows_per_chunk)) {
+    if (dstep_cross_attn_supported(1500, rows_per_chunk)) {
       DStepArgs xa{};
       xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
       xa.H = H; xa.T = 1500; xa.d = dt; xa.rows_per_chunk = rows_per_chunk; xa.n_chunks = n_chunks;
       dstep_cross_attn_launch(xa, l, s);
-    } else {
+    } else {  // more than 8 rows per chunk: prefill passes, beams above 8
       CrossAttnArgs ca;
       ca.q = m->d_q;
       ca.bind = m->d_bind;
       ca.layer = l;
       ca.out = m->d_ao; ca.partial = m->d_xpart; ca.counters = m->d_counters + 64;
-      ca.T = 1500; ca.H = H; ca.d = dt; ca.rows_per_chunk = rows_per_chunk; ca.splits = splits; ca.qgroups = qgroups;
+      ca.T = 1500; ca.H = H; ca.d = dt; ca.rows_per_chunk = rows_per_chunk; ca.splits = kXSplits; ca.qgroups = qgroups;
       dec_cross_attn(ca, n_chunks, s);
     }
     GvArgs ox;
@@ -958,15 +979,8 @@ static void logits_gemm(Model* m, int R) {
   gv(m, a);
 }
 
-static int pick_splits(const Model* m, int n_chunks, int rows_per_chunk) {
-  // 8 key splits (~188 keys each): the V tile fits in shared memory next to the scores and even one chunk fills the SMs
-  (void)m; (void)n_chunks; (void)rows_per_chunk;
-  return 8;
-}
-
 // Forced decoding of tokens[chunk][i0..i1) for chunks [chunk0, chunk0+n): rows = n*(i1-i0) <= 80, slot 0.
-static void prefill_pass(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int i0, int i1, int slots,
-                         int step_base) {
+static void prefill_pass(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int i0, int i1, int slots) {
   const int rpc = i1 - i0, R = n * rpc;
   std::vector<RowInfo> rows(R);
   std::vector<int> toks(R);
@@ -979,30 +993,17 @@ static void prefill_pass(Model* m, const Encoded* e, int chunk0, int n, const in
   B2W_CUDA(cudaMemcpyAsync(m->sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   B2W_CUDA(cudaStreamSynchronize(m->stream));  // host vectors go out of scope
   bind_encoded(m, e, chunk0);
-  decoder_layers(m, n, rpc, slots, pick_splits(m, n, rpc), step_base);
+  ensure_xpart(m, xpart_floats(m, n, rpc));
+  decoder_layers(m, n, rpc, slots);
 }
 
-struct HypOut {
-  std::vector<int> ids;
-  float score;
-};
-
-static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_t* prompts, int P, const b2w_gen_opts& o,
-                           int32_t* out_ids, int32_t* out_lens, float* out_scores, float* out_ns) {
+// ---- generate: one group of n chunks x K rows --------------------------------------------------------------------------------
+// Position of <|startoftranscript|>, which must be the same in every prompt of the group.
+static int validate_prompts(const Model* m, const int32_t* prompts, int n, int P) {
   const b2w_config& c = m->cfg;
-  const bool beam = o.beam_size > 1;
-  const int K = beam ? o.beam_size : std::max(1, o.num_hypotheses);
-  const int num_hyp = std::max(1, o.num_hypotheses);
-  const int R = n * K;
-  const int max_steps = o.max_length - P;
-  cudaStream_t s = m->stream;
-  const SearchBuffers& sb = m->sb;
-  const int n_ctx = c.n_text_ctx;
-
-  // ---- validate prompts / find SOT ----
   int sot_index = -1;
   for (int b = 0; b < n; ++b) {
-    const int32_t* p = prompts + (size_t)(chunk0 + b) * P;
+    const int32_t* p = prompts + (size_t)b * P;
     int si = -1;
     for (int i = 0; i < P; ++i) {
       B2W_CHECK(p[i] >= 0 && p[i] < c.n_vocab, "prompt token id out of range");
@@ -1012,24 +1013,27 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
     if (sot_index < 0) sot_index = si;
     else if (si != sot_index) throw Error("<|startoftranscript|> must be at the same position in all prompts", true);
   }
-  for (int b = 0; b < n; ++b) out_ns[chunk0 + b] = 0.f;
+  return sot_index;
+}
 
-  // ---- search parameters ----
+static SearchParams search_params(const Model* m, const int32_t* prompts, int n, int K, int P, int sot_index, const b2w_gen_opts& o) {
+  const b2w_config& c = m->cfg;
+  const bool beam = o.beam_size > 1;
   SearchParams sp{};
   sp.n_vocab = c.n_vocab; sp.vpad = m->vpad; sp.B = n; sp.K = K;
   sp.mode = beam ? 0 : 1;
   sp.ncand = beam ? 2 * K : 1;
-  sp.max_steps = max_steps; sp.prompt_len = P;
+  sp.max_steps = o.max_length - P; sp.prompt_len = P;
   sp.max_finished = std::max(1, (int)lroundf(K * o.patience));
   sp.allow_early_exit = (o.patience == 1.0f && o.length_penalty == 0.0f) ? 1 : 0;
-  sp.num_hyp = num_hyp;
+  sp.num_hyp = std::max(1, o.num_hypotheses);
   sp.length_penalty = o.length_penalty; sp.repetition_penalty = o.repetition_penalty;
   sp.no_repeat_ngram = o.no_repeat_ngram_size;
   sp.suppress_blank = o.suppress_blank;
   sp.n_suppress_begin = c.n_suppress_begin;
   for (int i = 0; i < 8; ++i) sp.suppress_begin[i] = c.suppress_begin[i];
   bool has_no_ts = false;
-  for (int i = 0; i < P; ++i) has_no_ts = has_no_ts || prompts[(size_t)chunk0 * P + i] == c.no_timestamps;
+  for (int i = 0; i < P; ++i) has_no_ts = has_no_ts || prompts[i] == c.no_timestamps;
   sp.timestamp_rules = has_no_ts ? 0 : 1;
   sp.max_initial_ts = o.max_initial_timestamp_index;
   sp.eot = c.eot; sp.no_timestamps = c.no_timestamps; sp.timestamp_begin = c.timestamp_begin; sp.no_speech = c.no_speech;
@@ -1038,41 +1042,57 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
   sp.want_no_speech_first = (o.return_no_speech_prob && sot_index == P - 1) ? 1 : 0;
   sp.fake_logits = o.debug_fake_logits;
   B2W_CHECK(sp.max_finished <= kMaxFinished, "beam_size * patience is too large");
+  return sp;
+}
 
-  if (max_steps <= 0) {
-    for (int b = 0; b < n; ++b)
-      for (int h = 0; h < num_hyp; ++h) {
-        out_lens[(size_t)(chunk0 + b) * num_hyp + h] = 0;
-        out_scores[(size_t)(chunk0 + b) * num_hyp + h] = 0.f;
-      }
-    return;
-  }
-
-  // ---- reset search state ----
-  const size_t RB = (size_t)n * K;
-  B2W_CUDA(cudaMemsetAsync(sb.state, 0, sizeof(SearchState), s));
-  B2W_CUDA(cudaMemsetAsync(sb.cum, 0, 2 * RB * 4, s));
-  B2W_CUDA(cudaMemsetAsync(sb.anc, 0, 2 * RB * n_ctx, s));
-  B2W_CUDA(cudaMemsetAsync(sb.done, 0, n * 4, s));
-  B2W_CUDA(cudaMemsetAsync(sb.fin_count, 0, n * 4, s));
-  B2W_CUDA(cudaMemsetAsync(sb.fin_len, 0xFF, (size_t)n * kMaxFinished * 4, s));
-  B2W_CUDA(cudaMemsetAsync(sb.no_speech, 0, n * 4, s));
-
-  // ---- prefill: prompt[:-1] in passes of <= 80 rows ----
-  if (!sp.fake_logits && P > 1) {
-    ScopedStage st(m, B2W_T_PREFILL);
-    const int per_pass = std::max(1, kMaxRows / n);
-    for (int i0 = 0; i0 < P - 1; i0 += per_pass) {
-      const int i1 = std::min(P - 1, i0 + per_pass);
-      prefill_pass(m, e, chunk0, n, prompts, P, i0, i1, K, P - 1);
-      if (o.return_no_speech_prob && sot_index >= i0 && sot_index < i1) {
-        logits_gemm(m, n * (i1 - i0));
-        no_speech_from_logits(m->d_logits, m->vpad, n * (i1 - i0), i1 - i0, sot_index - i0, c.n_vocab, c.no_speech, sb.no_speech, s);
-      }
+// Prompt[:-1] of every chunk in passes of <= 80 rows; the no-speech probability comes from the pass that holds the SOT row.
+static void prefill(Model* m, const Encoded* e, int chunk0, int n, const int32_t* prompts, int P, int K, int sot_index, bool no_speech) {
+  ScopedStage st(m, B2W_T_PREFILL);
+  const b2w_config& c = m->cfg;
+  const int per_pass = std::max(1, kMaxRows / n);
+  for (int i0 = 0; i0 < P - 1; i0 += per_pass) {
+    const int i1 = std::min(P - 1, i0 + per_pass);
+    prefill_pass(m, e, chunk0, n, prompts, P, i0, i1, K);
+    if (no_speech && sot_index >= i0 && sot_index < i1) {
+      logits_gemm(m, n * (i1 - i0));
+      no_speech_from_logits(m->d_logits, m->vpad, n * (i1 - i0), i1 - i0, sot_index - i0, c.n_vocab, c.no_speech, m->sb.no_speech, m->stream);
     }
   }
+}
 
-  // ---- decode rows ----
+struct Step {  // one decode step of a chunk group: its path and the argument block of a persistent kernel
+  StepPath path;
+  int n, K;
+  DStepArgs ds{};
+  BStepArgs bs{};
+};
+
+// The one step-path decision: fake logits when asked for, else the <= 8-row kernel, else the many-row kernel, else the layered
+// step.  B2W_STEP forces a path; a shape the forced kernel cannot take is an invalid argument.  Fills the shape of bs.
+static Step choose_step(const Model* m, int n, int K, bool fake_logits) {
+  const b2w_config& c = m->cfg;
+  Step st{StepPath::FakeLogits, n, K};
+  if (fake_logits) return st;
+  BStepArgs& bs = st.bs;
+  bs.L = c.n_text_layer; bs.w8 = m->w8 ? 1 : 0;
+  bs.R = n * K; bs.d = c.n_text_state; bs.H = c.n_text_head; bs.n_ctx = c.n_text_ctx; bs.slots = K; bs.T = 1500;
+  bs.vpad = m->vpad; bs.n_vocab = c.n_vocab; bs.n_chunks = n; bs.rows_per_chunk = K;
+  const bool dstep_ok = m->dstep_grid > 0 && n * K <= 8;
+  const bool bstep_ok = m->bstep_packed && bstep_supported(m->num_sms, bs);
+  st.path = m->forced_step.value_or(dstep_ok ? StepPath::Dstep : bstep_ok ? StepPath::Bstep : StepPath::Layers);
+  if ((st.path == StepPath::Dstep && !dstep_ok) || (st.path == StepPath::Bstep && !bstep_ok))
+    throw Error("B2W_STEP forces a step kernel that cannot run " + std::to_string(n) + " chunks x " + std::to_string(K) + " rows of this model",
+                true);
+  return st;
+}
+
+// Uploads the first decode rows, the search parameters and the encoder binding, sizes the partial buffer and binds the
+// workspace into the persistent kernel's argument block.
+static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const int32_t* prompts, int P, const SearchParams& sp) {
+  const b2w_config& c = m->cfg;
+  const int n = st.n, K = st.K, R = n * K;
+  cudaStream_t s = m->stream;
+  const SearchBuffers& sb = m->sb;
   {
     std::vector<RowInfo> rows(R);
     std::vector<int> toks(R);
@@ -1085,22 +1105,9 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
     B2W_CUDA(cudaMemcpyAsync(sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, s));
     B2W_CUDA(cudaStreamSynchronize(s));
   }
-  const int splits = pick_splits(m, n, K);
-  if (!sp.fake_logits) {
-    // lazily-grown partial buffer of the cross attention: sized before any kernel argument block captures the pointer
-    size_t need_part = cross_attn_partial_floats(n, c.n_text_head, K, splits);
-    need_part = std::max(need_part, (size_t)n * c.n_text_head * kDsXSplits * 8 * 66);
-    if (need_part > m->d_xpart_floats) {
-      B2W_CUDA(cudaStreamSynchronize(s));
-      if (m->d_xpart) cudaFree(m->d_xpart);
-      m->d_xpart = dalloc<float>(need_part);
-      m->d_xpart_floats = need_part;
-    }
-  }
-  // persistent single-kernel step for <= 8 rows
-  DStepArgs ds{};
-  bool use_dstep = m->use_dstep && !sp.fake_logits && R <= 8 && !m->use_ref_gemv && c.n_text_layer <= 32;
-  if (use_dstep) {
+  if (st.path != StepPath::FakeLogits) ensure_xpart(m, xpart_floats(m, n, K));
+  if (st.path == StepPath::Dstep) {
+    DStepArgs& ds = st.ds;
     ds.layers = m->d_layers; ds.L = c.n_text_layer; ds.tok_emb = m->tok_emb; ds.pos_emb = m->dec_pos;
     ds.logit_tiles = m->logit_tiles;
     ds.w8 = m->w8 ? 1 : 0;
@@ -1112,212 +1119,105 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
     ds.anc = sb.anc; ds.anc_buf_stride = (long long)n * K * c.n_text_ctx;
     ds.bind = m->d_bind; ds.xpart = m->d_xpart; ds.xcounters = m->d_counters + 64; ds.bar = m->d_bar;
     ds.prof = m->d_prof;
-    if (m->dstep_grid == 0) {
-      m->dstep_grid = dstep_max_grid(m->num_sms, ds);
-      if (m->dstep_grid == 0) m->dstep_grid = -1;
-    }
-    if (m->dstep_grid <= 0) use_dstep = false;
-  }
-  // persistent many-row step (bstep.cu) for everything the <= 8-row kernel does not take
-  BStepArgs bs{};
-  bool use_bstep = m->use_bstep && m->bstep_packed && !sp.fake_logits && !m->use_ref_gemv && (m->bstep_all || !use_dstep) && R <= kBsMaxRows;
-  if (use_bstep) {
-    bs.layers = m->d_blayers; bs.L = c.n_text_layer; bs.tok_emb = m->tok_emb; bs.pos_emb = m->dec_pos;
-    bs.logit_atoms = m->logit_atoms; bs.logit_bias = m->logit_b; bs.logit_scale = m->logit_scale; bs.w8 = m->w8 ? 1 : 0;
-    bs.R = R; bs.d = c.n_text_state; bs.H = c.n_text_head; bs.n_ctx = c.n_text_ctx; bs.slots = K; bs.T = 1500;
-    bs.vpad = m->vpad; bs.n_vocab = c.n_vocab; bs.n_chunks = n; bs.rows_per_chunk = K;
-    bs.stop_phase = m->bstep_stop;
-    if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // re-read per call: tools/bstep_bisect.py steps it
+  } else if (st.path == StepPath::Bstep) {
+    BStepArgs& bs = st.bs;
+    B2W_CHECK(bstep_xpart_floats(bs) <= m->d_xpart_floats, "cross-attention partial buffer");
+    bs.layers = m->d_blayers; bs.tok_emb = m->tok_emb; bs.pos_emb = m->dec_pos;
+    bs.logit_atoms = m->logit_atoms; bs.logit_bias = m->logit_b; bs.logit_scale = m->logit_scale;
+    if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // read per call: tools/bstep_bisect.py steps it
     bs.rows = sb.rows; bs.tokens_in = sb.tokens_in;
     bs.x = m->d_x; bs.qkv32 = m->d_qkv32; bs.cq32 = m->d_cq32; bs.h32 = m->d_h32; bs.ao = m->d_ao; bs.h16 = m->d_h16; bs.xn16 = m->d_xn16;
     bs.stats = m->d_stats; bs.stpart = m->d_stpart; bs.gpart = m->d_gpart; bs.logits = m->d_logits;
     bs.kcache = m->kcache; bs.vcache = m->vcache; bs.kv_layer_stride = (long long)m->kv_elems;
     bs.anc = sb.anc; bs.anc_buf_stride = (long long)n * K * c.n_text_ctx;
-    bs.bind = m->d_bind; bs.xcounters = m->d_counters + 64; bs.bar = m->d_bar; bs.prof = m->d_prof;
-    use_bstep = bstep_supported(m->num_sms, bs);
-    if (use_bstep) {
-      use_dstep = false;
-      const size_t need_part = std::max(bstep_xpart_floats(bs), cross_attn_partial_floats(n, c.n_text_head, K, splits));
-      if (need_part > m->d_xpart_floats) {
-        B2W_CUDA(cudaStreamSynchronize(s));
-        if (m->d_xpart) cudaFree(m->d_xpart);
-        m->d_xpart = dalloc<float>(need_part);
-        m->d_xpart_floats = need_part;
-      }
-      bs.xpart = m->d_xpart;
-    }
+    bs.bind = m->d_bind; bs.xpart = m->d_xpart; bs.xcounters = m->d_counters + 64; bs.bar = m->d_bar; bs.prof = m->d_prof;
   }
   m->h_params = sp;
   B2W_CUDA(cudaMemcpyAsync(const_cast<SearchParams*>(sb.params), &m->h_params, sizeof(SearchParams), cudaMemcpyHostToDevice, s));
   bind_encoded(m, e, chunk0);
-  auto record_step = [&]() {
-    if (sp.fake_logits) {
-      fake_logits(m->d_logits, R, sb, s);
-    } else {
-      if (use_bstep) {
-        bstep_launch(bs, m->num_sms, s);
-      } else if (use_dstep) {
-        dstep_launch(ds, m->dstep_grid, s);
-      } else {
-        decoder_layers(m, n, K, K, splits, P - 1);
-        logits_gemm(m, R);
-      }
-    }
-    search_rows(m->d_logits, R, m->vpad, sb, s);
-    search_update(n, sb, s);
-  };
+}
 
-  // one CUDA graph per (shape, options, buffers) — replayed every step, no per-step host parameters
-  // the graph depends only on shapes and workspace pointers: options and encoder-output bindings are read from
-  // device memory by the kernels, so one instantiated graph serves every window / chunk group of the same shape
-  std::vector<uint8_t> key(4 * sizeof(void*) + 8 * sizeof(int));
-  {
-    uint8_t* k = key.data();
-    const void* ptrs[4] = {m->kcache, m->sb_blob, m->d_xpart, m->d_logits};
-    memcpy(k, ptrs, sizeof ptrs); k += sizeof ptrs;
-    int misc[8] = {splits, m->use_ref_gemv ? 1 : 0, n, K, sp.fake_logits, use_dstep ? 1 : (use_bstep ? 3 : 0), bs.stop_phase, 0};
-    memcpy(k, misc, sizeof misc);
+static void record_step(Model* m, const Step& st) {
+  const int R = st.n * st.K;
+  switch (st.path) {
+    case StepPath::FakeLogits: fake_logits(m->d_logits, R, m->sb, m->stream); break;
+    case StepPath::Dstep: dstep_launch(st.ds, m->dstep_grid, m->stream); break;
+    case StepPath::Bstep: bstep_launch(st.bs, m->num_sms, m->stream); break;
+    case StepPath::Layers:
+      decoder_layers(m, st.n, st.K, st.K);
+      logits_gemm(m, R);
+      break;
   }
-  if (sp.fake_logits == 0) {
-    // make sure lazily-grown buffers exist before capture (capture forbids cudaMalloc/sync)
-    const size_t need_part = cross_attn_partial_floats(n, c.n_text_head, K, splits);
-    if (need_part > m->d_xpart_floats) {
-      if (m->d_xpart) cudaFree(m->d_xpart);
-      m->d_xpart = dalloc<float>(need_part);
-      m->d_xpart_floats = need_part;
-      const void* px = m->d_xpart;
-      memcpy(key.data() + 2 * sizeof(void*), &px, sizeof px);
-    }
+  search_rows(m->d_logits, R, m->vpad, m->sb, m->stream);
+  search_update(st.n, m->sb, m->stream);
+}
+
+// One CUDA graph per (shape, path, buffers), replayed every step with no per-step host parameters.  The graph depends only on
+// shapes and workspace pointers: options and encoder-output bindings are read from device memory by the kernels, so one
+// instantiated graph serves every window / chunk group of the same shape.  Returns the kernels one replay launches.
+static int64_t step_graph(Model* m, const Step& st) {
+  const StepGraphKey key{m->kcache, m->sb_blob, m->d_xpart, m->d_logits, st.n, st.K, (int)st.path, st.bs.stop_phase};
+  if (m->step_graph && m->step_graph_key == key) return m->step_graph_kernels;
+  if (m->step_graph) {
+    cudaGraphExecDestroy(m->step_graph);
+    m->step_graph = nullptr;
   }
   const int64_t launches_before = g_launches;
-  bool graph_ok = m->use_graph;
-  if (graph_ok && (!m->step_graph || m->step_graph_key != key)) {
-    if (m->step_graph) {
-      cudaGraphExecDestroy(m->step_graph);
-      m->step_graph = nullptr;
-    }
-    cudaGraph_t graph = nullptr;
-    B2W_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    try {
-      record_step();
-    } catch (...) {
-      cudaStreamEndCapture(s, &graph);
-      if (graph) cudaGraphDestroy(graph);
-      throw;
-    }
-    B2W_CUDA(cudaStreamEndCapture(s, &graph));
-    B2W_CUDA(cudaGraphInstantiate(&m->step_graph, graph, 0));
-    cudaGraphDestroy(graph);
-    m->step_graph_key = key;
+  cudaGraph_t graph = nullptr;
+  B2W_CUDA(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
+  try {
+    record_step(m, st);
+  } catch (...) {
+    cudaStreamEndCapture(m->stream, &graph);
+    if (graph) cudaGraphDestroy(graph);
+    throw;
   }
-  if (g_launches != launches_before) m->step_graph_kernels = g_launches - launches_before;  // recorded during capture
-  const int64_t per_step_kernels = m->step_graph_kernels;
+  B2W_CUDA(cudaStreamEndCapture(m->stream, &graph));
+  B2W_CUDA(cudaGraphInstantiate(&m->step_graph, graph, 0));
+  cudaGraphDestroy(graph);
+  m->step_graph_key = key;
+  m->step_graph_kernels = g_launches - launches_before;  // recorded, not launched
   g_launches = launches_before;
+  return m->step_graph_kernels;
+}
 
-  // ---- step loop: the host only polls the done counter ----
+// Replays the step graph until every chunk is done or max_steps is reached; the host only polls the done counter.
+static void decode_loop(Model* m, const Step& st, int P, int max_steps) {
+  const int64_t per_step_kernels = step_graph(m, st);
+  ScopedStage stage(m, B2W_T_DECODE);
+  const b2w_config& c = m->cfg;
+  const int n = st.n, R = st.n * st.K;
+  // the persistent kernels stream int8 weights with compute_type int8*: half the fp16 bytes; per-channel scales are negligible
+  const bool w8_stream = m->w8 && (st.path == StepPath::Dstep || st.path == StepPath::Bstep);
+  const int poll = 4;
   int steps_run = 0;
-  {
-    ScopedStage st(m, B2W_T_DECODE);
-    const int poll = 4;
-    for (int step = 0; step < max_steps; ++step) {
-      if (graph_ok) {
-        B2W_CUDA(cudaGraphLaunch(m->step_graph, s));
-        g_launches += per_step_kernels;
-      } else {
-        record_step();
-      }
-      ++steps_run;
-      // algorithmic bytes of this step: weights + beam-shared cross-KV + self-KV read so far
-      // (the persistent kernels stream int8 weights with compute_type int8*: half the fp16 bytes; per-channel scales are negligible)
-      m->decode_alg_bytes += ((m->w8 && (use_dstep || use_bstep)) ? 0.5 * m->dec_weight_bytes : m->dec_weight_bytes) +
-                             (double)n * c.n_text_layer * 2.0 * 1500 * c.n_text_state * 2.0 +
-                             (double)R * (P + step) * c.n_text_layer * 2.0 * c.n_text_state * 2.0;
-      if ((step % poll) == poll - 1 && step + 1 < max_steps) {
-        B2W_CUDA(cudaMemcpyAsync(m->h_pinned, &sb.state->n_done, sizeof(int), cudaMemcpyDeviceToHost, s));
-        B2W_CUDA(cudaStreamSynchronize(s));
-        if (m->h_pinned[0] >= n) break;
-      }
-    }
-    m->decode_steps += steps_run;
-    if (m->d_prof && use_bstep) {
-      B2W_CUDA(cudaStreamSynchronize(s));
-      const int L = c.n_text_layer, nstamps = 1 + 2 * (2 + 9 * L) + 1;
-      std::vector<unsigned long long> t(nstamps);
-      B2W_CUDA(cudaMemcpy(t.data(), m->d_prof, nstamps * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-      static const char* names[9] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1", "gelu", "ffn2"};
-      double work[9] = {0}, wait[9] = {0};
-      unsigned long long prev = t[2];
-      for (int l = 0; l < L; ++l)
-        for (int ph = 0; ph < 9; ++ph) {
-          const int bi = 1 + 2 * (1 + l * 9 + ph);
-          work[ph] += double(t[bi] - prev);
-          wait[ph] += double(t[bi + 1] - t[bi]);
-          prev = t[bi + 1];
-        }
-      const int bf = 1 + 2 * (1 + 9 * L);
-      fprintf(stderr, "[bstep prof] last step (R=%d): total %.1f us; embed %.1f us; final-LN %.1f us; logits %.1f us\n", R, (t[nstamps - 1] - t[0]) / 1e3,
-              (t[2] - t[0]) / 1e3, (t[bf] - prev) / 1e3, (t[nstamps - 1] - t[bf + 1]) / 1e3);
-      for (int ph = 0; ph < 9; ++ph)
-        fprintf(stderr, "[bstep prof]   %-10s work %.2f us  barrier wait %.2f us (CTA 0, mean over %d layers)\n", names[ph], work[ph] / L / 1e3,
-                wait[ph] / L / 1e3, L);
-      {
-        std::vector<unsigned long long> f(8 * 16);
-        B2W_CUDA(cudaMemcpy(f.data(), m->d_prof + 3000, f.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        B2W_CUDA(cudaMemset(m->d_prof + 3000, 0, f.size() * sizeof(unsigned long long)));
-        if (f[6 * 16 + 15] > 0)
-          fprintf(stderr, "[bstep prof]   self-attn cycles per 16-key block (CTA 0 warp 0): (unused) %.0f  issue+copy-wait %.0f  compute %.0f; prologue per task total %.0f over %llu blocks\n",
-                  (double)f[6 * 16 + 1] / f[6 * 16 + 15], (double)f[6 * 16 + 2] / f[6 * 16 + 15], (double)f[6 * 16 + 3] / f[6 * 16 + 15], (double)f[6 * 16],
-                  f[6 * 16 + 15]);
-        if (f[7 * 16 + 15] > 0)
-          fprintf(stderr, "[bstep prof]   cross-attn cycles per tile (CTA 0): tile-wait %.0f  compute %.0f; piece ends total %.0f, prologues total %.0f over %llu tiles\n",
-                  (double)f[7 * 16] / f[7 * 16 + 15], (double)f[7 * 16 + 1] / f[7 * 16 + 15], (double)f[7 * 16 + 2], (double)f[7 * 16 + 3], f[7 * 16 + 15]);
-        static const char* kinds[6] = {"qkv", "out", "cross_q", "cross_out", "ffn1", "ffn2"};
-        for (int k = 0; k < 6; ++k) {
-          const double cnt = (double)f[k * 16 + 15];
-          if (cnt > 0)
-            fprintf(stderr, "[bstep prof]   %-9s cycles (CTA 0): stage %.0f  sync %.0f  row statistics %.0f  products + reduction %.0f\n", kinds[k],
-                    f[k * 16] / cnt, f[k * 16 + 4] / cnt, f[k * 16 + 5] / cnt, f[k * 16 + 2] / cnt);
-        }
-      }
-    }
-    if (m->d_prof && use_dstep) {
-      B2W_CUDA(cudaStreamSynchronize(s));
-      const int L = c.n_text_layer, nstamps = 1 + 2 * (1 + 8 * L) + 1;
-      std::vector<unsigned long long> t(nstamps);
-      B2W_CUDA(cudaMemcpy(t.data(), m->d_prof, nstamps * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-      // stamps: [0]=start, then (arrive, release) per barrier, then end.  work(p) = arrive_p - release_{p-1}; wait(p) = release_p - arrive_p
-      static const char* names[8] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1", "ffn2"};
-      double work[8] = {0}, wait[8] = {0};
-      unsigned long long prev = t[2];  // release of the embed barrier
-      for (int l = 0; l < L; ++l)
-        for (int ph = 0; ph < 8; ++ph) {
-          const int bi = 1 + 2 * (1 + l * 8 + ph);
-          work[ph] += double(t[bi] - prev);
-          wait[ph] += double(t[bi + 1] - t[bi]);
-          prev = t[bi + 1];
-        }
-      fprintf(stderr, "[dstep prof] last step: total %.1f us; embed %.1f us; logits %.1f us\n", (t[nstamps - 1] - t[0]) / 1e3,
-              (t[2] - t[0]) / 1e3, (t[nstamps - 1] - prev) / 1e3);
-      {
-        std::vector<unsigned long long> f(8 * 16);
-        B2W_CUDA(cudaMemcpy(f.data(), m->d_prof + 3000, f.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        B2W_CUDA(cudaMemset(m->d_prof + 3000, 0, f.size() * sizeof(unsigned long long)));
-        static const char* kinds[7] = {"qkv", "out", "cross_q", "cross_out", "ffn1", "ffn2", "logits"};
-        for (int k = 0; k < 7; ++k) {
-          const double n = (double)f[k * 16 + 15];
-          if (n > 0)
-            fprintf(stderr, "[dstep prof]   %-9s cycles (first item): stage-input %.0f  tile-wait %.0f  mma %.0f  epilogue %.0f\n", kinds[k], f[k * 16] / n,
-                    f[k * 16 + 1] / n, f[k * 16 + 2] / n, f[k * 16 + 3] / n);
-        }
-      }
-      for (int ph = 0; ph < 8; ++ph)
-        fprintf(stderr, "[dstep prof]   %-10s work %.2f us  barrier wait %.2f us (CTA 0, mean over %d layers)\n", names[ph], work[ph] / L / 1e3,
-                wait[ph] / L / 1e3, L);
+  for (int step = 0; step < max_steps; ++step) {
+    B2W_CUDA(cudaGraphLaunch(m->step_graph, m->stream));
+    g_launches += per_step_kernels;
+    ++steps_run;
+    // algorithmic bytes of this step: weights + beam-shared cross-KV + self-KV read so far
+    m->decode_alg_bytes += (w8_stream ? 0.5 * m->dec_weight_bytes : m->dec_weight_bytes) +
+                           (double)n * c.n_text_layer * 2.0 * 1500 * c.n_text_state * 2.0 +
+                           (double)R * (P + step) * c.n_text_layer * 2.0 * c.n_text_state * 2.0;
+    if ((step % poll) == poll - 1 && step + 1 < max_steps) {
+      B2W_CUDA(cudaMemcpyAsync(m->h_pinned, &m->sb.state->n_done, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+      B2W_CUDA(cudaStreamSynchronize(m->stream));
+      if (m->h_pinned[0] >= n) break;
     }
   }
+  m->decode_steps += steps_run;
+  if (m->d_prof && st.path == StepPath::Bstep) bstep_print_profile(st.bs, m->stream);
+  if (m->d_prof && st.path == StepPath::Dstep) dstep_print_profile(st.ds, m->stream);
+}
 
-  // ---- collect hypotheses ----
+// Finished hypotheses of every chunk, best first by (length-penalised) score.
+static void collect_hypotheses(Model* m, int chunk0, int n, int K, const b2w_gen_opts& o, int32_t* out_ids, int32_t* out_lens,
+                               float* out_scores, float* out_ns) {
   ScopedStage st(m, B2W_T_D2H);
+  cudaStream_t s = m->stream;
+  const SearchBuffers& sb = m->sb;
+  const int n_ctx = m->cfg.n_text_ctx, num_hyp = std::max(1, o.num_hypotheses);
+  const bool beam = o.beam_size > 1;
   std::vector<int> fin_count(n), fin_len((size_t)n * kMaxFinished);
   std::vector<float> fin_score((size_t)n * kMaxFinished), ns(n);
   std::vector<int> fin_tok((size_t)n * kMaxFinished * n_ctx);
@@ -1356,6 +1256,59 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
         out_lens[oi] = 0;
         out_scores[oi] = 0.f;
       }
+    }
+  }
+}
+
+static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_t* prompts, int P, const b2w_gen_opts& o,
+                           int32_t* out_ids, int32_t* out_lens, float* out_scores, float* out_ns) {
+  const int K = o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
+  const int sot_index = validate_prompts(m, prompts + (size_t)chunk0 * P, n, P);
+  for (int b = 0; b < n; ++b) out_ns[chunk0 + b] = 0.f;
+  const SearchParams sp = search_params(m, prompts + (size_t)chunk0 * P, n, K, P, sot_index, o);
+  Step st = choose_step(m, n, K, sp.fake_logits);
+  if (sp.max_steps <= 0) {
+    const int num_hyp = std::max(1, o.num_hypotheses);
+    for (int b = 0; b < n; ++b)
+      for (int h = 0; h < num_hyp; ++h) {
+        out_lens[(size_t)(chunk0 + b) * num_hyp + h] = 0;
+        out_scores[(size_t)(chunk0 + b) * num_hyp + h] = 0.f;
+      }
+    return;
+  }
+
+  // reset the search state
+  const SearchBuffers& sb = m->sb;
+  cudaStream_t s = m->stream;
+  const size_t RB = (size_t)n * K;
+  B2W_CUDA(cudaMemsetAsync(sb.state, 0, sizeof(SearchState), s));
+  B2W_CUDA(cudaMemsetAsync(sb.cum, 0, 2 * RB * 4, s));
+  B2W_CUDA(cudaMemsetAsync(sb.anc, 0, 2 * RB * m->cfg.n_text_ctx, s));
+  B2W_CUDA(cudaMemsetAsync(sb.done, 0, n * 4, s));
+  B2W_CUDA(cudaMemsetAsync(sb.fin_count, 0, n * 4, s));
+  B2W_CUDA(cudaMemsetAsync(sb.fin_len, 0xFF, (size_t)n * kMaxFinished * 4, s));
+  B2W_CUDA(cudaMemsetAsync(sb.no_speech, 0, n * 4, s));
+
+  if (!sp.fake_logits && P > 1) prefill(m, e, chunk0, n, prompts, P, K, sot_index, o.return_no_speech_prob);
+  bind_step(m, st, e, chunk0, prompts, P, sp);
+  decode_loop(m, st, P, sp.max_steps);
+  collect_hypotheses(m, chunk0, n, K, o, out_ids, out_lens, out_scores, out_ns);
+}
+
+// Debug / measurement switches, read once when a model is created (B2W_BSTEP_STOP is read per generate call, in bind_step).
+static void read_env_options(Model* m) {
+  if (const char* v = getenv("B2W_GEMM_IMPL")) m->use_ref_gemm = !strcmp(v, "ref");
+  if (const char* v = getenv("B2W_ATTN_IMPL")) m->use_ref_attn = !strcmp(v, "ref");
+  if (const char* v = getenv("B2W_STEP")) {
+    if (!strcmp(v, "dstep")) m->forced_step = StepPath::Dstep;
+    else if (!strcmp(v, "bstep")) m->forced_step = StepPath::Bstep;
+    else if (!strcmp(v, "layers")) m->forced_step = StepPath::Layers;
+    else if (*v) throw Error(std::string("B2W_STEP must be dstep, bstep or layers, not ") + v, true);
+  }
+  if (const char* v = getenv("B2W_DSTEP_PROF")) {
+    if (strcmp(v, "0") != 0) {
+      m->d_prof = model_alloc<unsigned long long>(m, 4096);
+      B2W_CUDA(cudaMemset(m->d_prof, 0, 4096 * sizeof(unsigned long long)));
     }
   }
 }
@@ -1418,32 +1371,8 @@ int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n
     B2W_CUDA(cudaGetDeviceProperties(&prop, device));
     m->num_sms = prop.multiProcessorCount;
     B2W_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
-    if (const char* v = getenv("B2W_GEMM_IMPL")) m->use_ref_gemm = !strcmp(v, "ref");
-    if (const char* v = getenv("B2W_ATTN_IMPL")) m->use_ref_attn = !strcmp(v, "ref");
-    if (const char* v = getenv("B2W_GEMV_IMPL")) m->use_ref_gemv = !strcmp(v, "ref");
-    if (const char* v = getenv("B2W_GRAPH")) m->use_graph = strcmp(v, "0") != 0;
     m->w8 = ct.rfind("int8", 0) == 0;
-    if (const char* v = getenv("B2W_W8_FAKE")) {
-      if (strcmp(v, "0") != 0) {
-        m->w8_fake = true;
-        m->w8 = false;
-      }
-    }
-    if (const char* v = getenv("B2W_DSTEP")) {
-      m->use_dstep = strcmp(v, "0") != 0;
-    }
-    if (const char* v = getenv("B2W_BSTEP")) {
-      m->use_bstep = strcmp(v, "0") != 0;
-      m->bstep_all = strcmp(v, "all") == 0;
-    }
-    if (const char* v = getenv("B2W_BSTEP_STOP")) m->bstep_stop = atoi(v);
-    if (const char* v = getenv("B2W_XATTN_IMPL")) m->use_mma_xattn = strcmp(v, "simt") != 0;
-    if (const char* v = getenv("B2W_DSTEP_PROF")) {
-      if (strcmp(v, "0") != 0) {
-        m->d_prof = dalloc<unsigned long long>(4096);
-        B2W_CUDA(cudaMemset(m->d_prof, 0, 4096 * sizeof(unsigned long long)));
-      }
-    }
+    read_env_options(m);
     TensorTable tt{tensors, n_tensors};
     build_model(m, *cfg, tt);
     *out = h.release();
@@ -1684,7 +1613,7 @@ int b2w_detect_language(b2w_model* h, b2w_encoded* enc, float* probs) {
     for (int c0 = 0; c0 < e->B; c0 += group) {
       const int n = std::min(group, e->B - c0);
       B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * m->cfg.n_text_ctx, m->stream));
-      prefill_pass(m, e, c0, n, toks.data(), 1, 0, 1, 1, 0);
+      prefill_pass(m, e, c0, n, toks.data(), 1, 0, 1, 1);
       logits_gemm(m, n);
       lang_probs_from_logits(m->d_logits, m->vpad, n, m->cfg.lang_begin, nl, d_probs + (size_t)c0 * nl, m->stream);
     }
@@ -1828,7 +1757,7 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
       for (int i0 = 0; i0 < n_tok; i0 += kMaxRows) {
         const int i1 = std::min(n_tok, i0 + kMaxRows);
         m->align_pos0 = i0;
-        prefill_pass(m, e, batch_index, 1, padded.data(), n_tok, i0, i1, 1, 0);
+        prefill_pass(m, e, batch_index, 1, padded.data(), n_tok, i0, i1, 1);
         logits_gemm(m, i1 - i0);
         row_target_probs(m->d_logits, m->vpad, i1 - i0, c.n_vocab, d_targets + i0, d_tp + i0, s);
       }
@@ -2090,7 +2019,7 @@ int b2w_debug_logits(b2w_model* h, b2w_encoded* enc, const int32_t* tokens, int3
       const int per_pass = std::max(1, kMaxRows / n);
       for (int i0 = 0; i0 < n_tok; i0 += per_pass) {
         const int i1 = std::min((int)n_tok, i0 + per_pass), rpc = i1 - i0;
-        prefill_pass(m, e, c0, n, tokens, n_tok, i0, i1, 1, 0);
+        prefill_pass(m, e, c0, n, tokens, n_tok, i0, i1, 1);
         logits_gemm(m, n * rpc);
         B2W_CUDA(cudaMemcpyAsync(tmp.data(), m->d_logits, (size_t)n * rpc * m->vpad * 4, cudaMemcpyDeviceToHost, m->stream));
         B2W_CUDA(cudaStreamSynchronize(m->stream));

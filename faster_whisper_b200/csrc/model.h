@@ -3,6 +3,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -38,6 +39,11 @@ struct StageTimer {
   cudaEvent_t start, stop;
 };
 
+// The decode step runs as the layered multi-kernel sequence or as one of the two persistent kernels; B2W_STEP forces one.
+enum class StepPath { Layers, Dstep, Bstep, FakeLogits };
+// kcache, sb_blob, d_xpart, d_logits, chunks, rows per chunk, path, B2W_BSTEP_STOP
+using StepGraphKey = std::tuple<const void*, const void*, const void*, const void*, int, int, int, int>;
+
 struct Model;
 
 struct Encoded {
@@ -57,7 +63,7 @@ struct Model {
   int vpad = 0;     // vocabulary padded to a multiple of 16
   cudaStream_t stream = nullptr;
   std::mutex mu;
-  std::vector<void*> allocs;  // weights
+  std::vector<void*> allocs;  // allocated once (weights, decoder workspace), freed with the model
   // size-keyed free list for encoder outputs / cross-KV caches: a 3.9 GB cudaMalloc+cudaFree per call costs ~100s of ms
   std::vector<std::pair<size_t, void*>> pool;
   size_t pool_bytes = 0;
@@ -120,24 +126,19 @@ struct Model {
   const __half* logit_tiles = nullptr;  // output embedding as the persistent step kernel's tile stream
   DLayer* d_layers = nullptr;   // device copy of the decoder layer pointer table (persistent step kernel)
   unsigned* d_bar = nullptr;
-  unsigned long long* d_prof = nullptr;  // B2W_DSTEP_PROF=1: per-phase timestamps of the persistent step kernel
-  int dstep_grid = 0;
+  unsigned long long* d_prof = nullptr;  // B2W_DSTEP_PROF=1: per-phase timestamps of the persistent step kernels
+  int dstep_grid = 0;  // grid of the <= 8-row step kernel (dstep.cu); 0 when it cannot run this model
   // compute_type int8*: the decoder's linear layers (and the output embedding) are quantised per output channel; the persistent step
-  // kernel streams them as int8 (w8), every other path uses the de-quantised fp16 values.  w8_fake keeps fp16 tiles of the same
-  // de-quantised values (B2W_W8_FAKE=1: the reference the int8 stream is tested against).
-  bool w8 = false, w8_fake = false;
-  bool use_dstep = true;
+  // kernels stream them as int8 (w8), every other path uses the de-quantised fp16 values.
+  bool w8 = false;
   // many-row persistent step kernel (bstep.cu): decoder weights as 16 KB wgmma atoms + per-row sums for the deferred LayerNorm
-  bool use_bstep = true;     // B2W_BSTEP=0 falls back to the multi-kernel step for R > 8
-  bool bstep_all = false;    // B2W_BSTEP=all: also for R <= 8 (instead of dstep_kernel)
-  int bstep_stop = 0;        // B2W_BSTEP_STOP=n: run only the first n grid phases of every step (debug)
   bool bstep_packed = false;
   BLayer* d_blayers = nullptr;
   const void* logit_atoms = nullptr;
   const float* logit_scale = nullptr;
   float *d_qkv32 = nullptr, *d_cq32 = nullptr, *d_h32 = nullptr, *d_stats = nullptr, *d_gpart = nullptr, *d_stpart = nullptr;
   __half *d_h16 = nullptr, *d_xn16 = nullptr;
-  bool use_mma_xattn = true;  // decode cross attention on mma.sync (dstep.cu) instead of the SIMT kernel (B2W_XATTN_IMPL=simt)
+  std::optional<StepPath> forced_step;  // B2W_STEP=dstep|bstep|layers (tests and tools)
   DecBindings h_bind{};
   SearchParams h_params{};
   // search buffers
@@ -149,7 +150,7 @@ struct Model {
   // step graph cache
   cudaGraphExec_t step_graph = nullptr;
   int64_t step_graph_kernels = 0;
-  std::vector<uint8_t> step_graph_key;
+  StepGraphKey step_graph_key{};
 
   // measurement
   bool timing = false;
@@ -159,7 +160,7 @@ struct Model {
   int64_t launches = 0, decode_steps = 0;
   double decode_alg_bytes = 0;
 
-  bool use_ref_gemm = false, use_ref_attn = false, use_ref_gemv = false, use_graph = true;
+  bool use_ref_gemm = false, use_ref_attn = false;
 
   ~Model();
 };

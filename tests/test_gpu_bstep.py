@@ -84,9 +84,9 @@ def test_batched_decode_multilingual_geometry(micro_ml):
 
 @pytest.mark.parametrize("n_chunks,beam", [(1, 5), (3, 1), (1, 1)])
 def test_many_row_kernel_on_few_rows(micro_ml, n_chunks, beam):
-    """B2W_BSTEP=all routes R <= 8 through the many-row kernel too (wgmma N = 16): same tokens as the oracle."""
+    """B2W_STEP=bstep routes R <= 8 through the many-row kernel too (wgmma N = 16): same tokens as the oracle."""
     st = micro_ml["tokens"]
-    eng = make_engine(micro_ml, B2W_BSTEP="all")
+    eng = make_engine(micro_ml, B2W_STEP="bstep")
     feats = features_for(micro_ml, n_chunks, seed=310)
     prompts = [[st.sot_prev, 700, 701, st.sot, st.lang_begin, st.transcribe]] * n_chunks
     exact, n = compare(eng, micro_ml, feats, prompts, beam_size=beam, max_length=40, repetition_penalty=1.2, no_repeat_ngram_size=3)
@@ -94,13 +94,13 @@ def test_many_row_kernel_on_few_rows(micro_ml, n_chunks, beam):
 
 
 def test_many_row_kernel_matches_multikernel_path(micro):
-    """Same call through the persistent kernel and through the round-1 multi-kernel graph (B2W_BSTEP=0)."""
+    """Same call through the persistent kernel and through the layered multi-kernel step (B2W_STEP=layers)."""
     st = micro["tokens"]
     feats = features_for(micro, 6, seed=320)
     prompts = [[st.sot, st.no_timestamps]] * 6
     kw = dict(beam_size=5, max_length=30, return_scores=True, repetition_penalty=1.25, no_repeat_ngram_size=3, suppress_tokens=[st.eot])
-    a = make_engine(micro)
-    b = make_engine(micro, B2W_BSTEP="0")
+    a = make_engine(micro, B2W_STEP="bstep")
+    b = make_engine(micro, B2W_STEP="layers")
     ra = a.generate(a.encode(feats), prompts, **kw)
     rb = b.generate(b.encode(feats), prompts, **kw)
     same = sum(x.sequences_ids[0] == y.sequences_ids[0] for x, y in zip(ra, rb))
@@ -118,7 +118,7 @@ def test_many_row_kernel_long_context(micro_ml, n_chunks, beam, late):
     greedy rows are checked exactly: a row may part from the oracle only at a step where the oracle's own top-1 / top-2 gap is below
     twice the logit tolerance (compare() looks the gap up at that very step), and most rows must run the whole length identical."""
     st = micro_ml["tokens"]
-    eng = make_engine(micro_ml, B2W_BSTEP="all")
+    eng = make_engine(micro_ml, B2W_STEP="bstep")
     feats = features_for(micro_ml, n_chunks, seed=330)
     prompts = [[st.sot, st.lang_begin, st.transcribe, st.no_timestamps]] * n_chunks
     exact, n = compare(eng, micro_ml, feats, prompts, beam_size=beam, max_length=240, suppress_tokens=[st.eot], repetition_penalty=1.3, no_repeat_ngram_size=3)
@@ -157,3 +157,33 @@ def test_repeated_batched_steps_are_bit_identical(micro_ml):
     assert t0 == t1 and s0 == s1
     for name, x, y in zip(("residual stream", "LayerNorm statistics", "logits"), b0, b1):
         assert np.array_equal(x, y), (name, np.abs(x - y).max())
+
+
+def test_forced_step_runs_the_path_it_names(micro_ml, capfd):
+    """B2W_STEP forces one decode-step path.  A shape the forced kernel cannot take is a ValueError, not a fallback.  Each setting
+    runs what it names: with a prompt of [sot] there is no prefill, and a second generate() over the same encoder output computes
+    no cross-attention K/V, so the launches counted per step are those of one step graph — O(L) kernels for the layered step, the
+    same constant number for both persistent kernels, which tell themselves apart by the profile they print (B2W_DSTEP_PROF)."""
+    st, L = micro_ml["tokens"], micro_ml["dims"].n_text_layer
+    feats = features_for(micro_ml, 2, seed=350)
+    kw = dict(beam_size=2, max_length=12, suppress_tokens=[st.eot])
+    per_step = {}
+    for path in ("dstep", "bstep", "layers"):
+        eng = make_engine(micro_ml, B2W_STEP=path, B2W_DSTEP_PROF="1")
+        if path == "dstep":
+            with pytest.raises(ValueError):
+                eng.generate(eng.encode(feats), [[st.sot]] * 2, beam_size=5, max_length=8)  # 2 chunks x beam 5 = 10 rows
+        if path == "bstep":
+            with pytest.raises(ValueError):
+                eng.generate(eng.encode(feats), [[st.sot]] * 2, beam_size=9, max_length=8)  # 9 rows per chunk
+        enc = eng.encode(feats[:1])
+        eng.generate(enc, [[st.sot]], **kw)
+        capfd.readouterr()
+        eng.timing(reset=True)
+        eng.generate(enc, [[st.sot]], **kw)
+        t, err = eng.timing(), capfd.readouterr().err
+        assert t["decode_steps"] > 0 and t["launches"] % t["decode_steps"] == 0, t
+        per_step[path] = t["launches"] // t["decode_steps"]
+        assert ("[dstep prof]" in err) == (path == "dstep") and ("[bstep prof]" in err) == (path == "bstep"), (path, err[:300])
+    assert per_step["dstep"] == per_step["bstep"], per_step
+    assert per_step["layers"] >= per_step["dstep"] + 8 * L, per_step  # per layer: 4 projections, 2 attentions, 2 FFN GEMMs

@@ -203,25 +203,26 @@ def test_generate_errors(micro, eng):
     assert r[0].sequences_ids == [[]]
 
 
-# ---- persistent single-kernel decode step (R <= 8 rows) vs the multi-kernel path and the oracle --------------------------
+# ---- persistent single-kernel decode step (R <= 8 rows) vs the many-row kernel, the multi-kernel path and the oracle ------------
 @pytest.mark.parametrize("beam,n_chunks", [(5, 1), (1, 1), (1, 4), (2, 3), (1, 8)])  # (1, 8): 168 cross-attention tasks > 132 CTAs
 def test_persistent_step_matches_multikernel_path(micro_ml, beam, n_chunks):
     st = micro_ml["tokens"]
     feats = features_for(micro_ml, n_chunks, seed=90)
     prompts = [[st.sot_prev, 700, 701, st.sot, st.lang_begin, st.transcribe]] * n_chunks
     kw = dict(beam_size=beam, max_length=40, return_scores=True, return_no_speech_prob=True, repetition_penalty=1.2, no_repeat_ngram_size=3)
-    fused = make_engine(micro_ml, B2W_DSTEP="1")
-    split = make_engine(micro_ml, B2W_DSTEP="0")
-    a = fused.generate(fused.encode(feats), prompts, **kw)
-    b = split.generate(split.encode(feats), prompts, **kw)
+    res = {}
+    for path in ("dstep", "bstep", "layers"):
+        e = make_engine(micro_ml, B2W_STEP=path)
+        res[path] = e.generate(e.encode(feats), prompts, **kw)
     o = micro_ml["oracle"]
     want = o.generate(o.encode(feats), prompts, **{k: v for k, v in kw.items()})
-    for x, y, w in zip(a, b, want):
-        if x.sequences_ids[0] != y.sequences_ids[0] or x.sequences_ids[0] != w.sequences_ids[0]:
-            assert w.min_margin < 2 * LOGIT_TOL, (w.min_margin, x.sequences_ids[0][:10], y.sequences_ids[0][:10], w.sequences_ids[0][:10])
-        else:
-            assert abs(x.scores[0] - y.scores[0]) < 2e-3 and abs(x.scores[0] - w.scores[0]) < 0.05
-        assert abs(x.no_speech_prob - w.no_speech_prob) < 5e-3 * max(1.0, w.no_speech_prob) + 1e-6
+    for other in ("bstep", "layers"):
+        for x, y, w in zip(res["dstep"], res[other], want):
+            if x.sequences_ids[0] != y.sequences_ids[0] or x.sequences_ids[0] != w.sequences_ids[0]:
+                assert w.min_margin < 2 * LOGIT_TOL, (other, w.min_margin, x.sequences_ids[0][:10], y.sequences_ids[0][:10], w.sequences_ids[0][:10])
+            else:
+                assert abs(x.scores[0] - y.scores[0]) < 2e-3 and abs(x.scores[0] - w.scores[0]) < 0.05, other
+            assert abs(x.no_speech_prob - w.no_speech_prob) < 5e-3 * max(1.0, w.no_speech_prob) + 1e-6
 
 
 # ---- Whisper.align (word timestamps): cross-attention capture + DTW vs the oracle ---------------------------------------------
@@ -371,15 +372,15 @@ def test_in_process_replicas_on_two_gpus(micro_ml):
 
 
 def test_persistent_step_long_context(micro_ml):
-    """More than kDsSelfKeys (192) cached positions: the persistent kernel's multi-pass self-attention with online softmax."""
+    """More than kDsSelfKeys (192) cached positions: the persistent kernels' multi-pass self-attention with online softmax."""
     st = micro_ml["tokens"]
     feats = features_for(micro_ml, 1, seed=95)
     prompts = [[st.sot, st.lang_begin, st.transcribe, st.no_timestamps]]
     kw = dict(beam_size=1, max_length=240, return_scores=True, suppress_tokens=[st.eot], repetition_penalty=1.3, no_repeat_ngram_size=3)
-    fused = make_engine(micro_ml, B2W_DSTEP="1")
-    split = make_engine(micro_ml, B2W_DSTEP="0")
-    a = fused.generate(fused.encode(feats), prompts, **kw)[0]
-    b = split.generate(split.encode(feats), prompts, **kw)[0]
+    few_rows = make_engine(micro_ml, B2W_STEP="dstep")
+    many_rows = make_engine(micro_ml, B2W_STEP="bstep")
+    a = few_rows.generate(few_rows.encode(feats), prompts, **kw)[0]
+    b = many_rows.generate(many_rows.encode(feats), prompts, **kw)[0]
     o = micro_ml["oracle"]
     w = o.generate(o.encode(feats), prompts, **kw)[0]
     assert len(w.sequences_ids[0]) == 236

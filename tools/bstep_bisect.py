@@ -1,7 +1,7 @@
 """Phase-by-phase check of the many-row persistent step kernel (csrc/bstep.cu) on a GPU box.
 
 Runs ONE decode step (prompt [sot, notimestamps], so the step feeds position 1 after a one-token prefill) with
-B2W_BSTEP=all and B2W_BSTEP_STOP=p for p = 1 .. number of grid phases, fetches the decoder workspace after each
+B2W_STEP=bstep and B2W_BSTEP_STOP=p for p = 1 .. number of grid phases, fetches the decoder workspace after each
 stop (b2w_debug_fetch) and compares it with a NumPy restatement of the same step.  Prints the max abs error per
 phase so one run bisects a wrong kernel.  Test infrastructure (imports oracle/ only for the log-mel features).
 
@@ -94,7 +94,7 @@ def main():
     ap.add_argument("--first", type=int, default=1)
     ap.add_argument("--last", type=int, default=0)
     args = ap.parse_args()
-    os.environ["B2W_BSTEP"] = "all"
+    os.environ["B2W_STEP"] = "bstep"
     from faster_whisper_b200 import engine
     from faster_whisper_b200.config import special_tokens
     from faster_whisper_b200.synthetic import custom_dims, make_weights, synthetic_audio

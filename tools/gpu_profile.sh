@@ -17,5 +17,5 @@ if [ -f faster_whisper_b200/libb200whisper_ticks.so ]; then
   B2W_LIBRARY=$PWD/faster_whisper_b200/libb200whisper_ticks.so timeout -s KILL 300 python tools/step_ab.py --batch 1 --repeat 1 --prof > gpurun_out/step_prof_single.log 2>&1; echo "step_prof single exit $?"
   grep "dstep prof\|decode" gpurun_out/step_prof_single.log | tail -n 16 | cut -c1-260
 fi
-timeout -s KILL 300 python tools/step_ab.py --batch 1 --configs "none;B2W_BSTEP=all" > gpurun_out/step_single_ab.log 2>&1; echo "single ab exit $?"; grep decode gpurun_out/step_single_ab.log | cut -c1-200
+timeout -s KILL 300 python tools/step_ab.py --batch 1 --configs "B2W_STEP=dstep;B2W_STEP=bstep" 2>&1 | grep decode | cut -c1-200; echo "single ab exit ${PIPESTATUS[0]}"
 ls -la gpurun_out/*.ncu-rep
