@@ -835,9 +835,10 @@ static void ensure_cross_kv(Model* m, Encoded* e) {
 
 constexpr int kTcMinRows = 17;  // rows above which the decode GEMMs go through the wgmma path (activations reused from smem)
 
-// decode GEMM through the tensor-core GEMM: the plan (TMA maps) is cached per (weights, activations, rows)
+// decode GEMM through the tensor-core GEMM: the plan (TMA maps and the epilogue's pointers) is cached per Model::dec_plans key
 static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
-  const auto key = std::make_tuple((const void*)a.W, (const void*)a.x, a.R, a.mode);
+  const auto key = std::make_tuple((const void*)a.W, (const void*)a.x, a.R, a.mode, (const void*)a.rows, (const void*)a.kcache,
+                                   (const void*)a.vcache, a.slots);
   auto it = m->dec_plans.find(key);
   if (it != m->dec_plans.end()) return it->second;
   GemmArgs g;
@@ -1137,7 +1138,8 @@ static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const in
   bind_encoded(m, e, chunk0);
 }
 
-static void record_step(Model* m, const Step& st) {
+// The decoder half of a step: the logits of every row into d_logits, from sb.rows, sb.tokens_in and sb.anc.
+static void launch_decoder(Model* m, const Step& st) {
   const int R = st.n * st.K;
   switch (st.path) {
     case StepPath::FakeLogits: fake_logits(m->d_logits, R, m->sb, m->stream); break;
@@ -1148,6 +1150,11 @@ static void record_step(Model* m, const Step& st) {
       logits_gemm(m, R);
       break;
   }
+}
+
+static void record_step(Model* m, const Step& st) {
+  const int R = st.n * st.K;
+  launch_decoder(m, st);
   search_rows(m->d_logits, R, m->vpad, m->sb, m->stream);
   search_update(st.n, m->sb, m->stream);
 }
@@ -2004,6 +2011,7 @@ int b2w_debug_logits(b2w_model* h, b2w_encoded* enc, const int32_t* tokens, int3
     B2W_CHECK(h && enc && enc->e && tokens && logits_out && enc->e->B == batch, "bad arguments");
     Model* m = &h->m;
     B2W_CHECK(n_tok >= 1 && n_tok <= m->cfg.n_text_ctx, "token count");
+    for (size_t i = 0; i < (size_t)batch * n_tok; ++i) B2W_CHECK(tokens[i] >= 0 && tokens[i] < m->cfg.n_vocab, "token id out of range");
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard g(m->device);
     Encoded* e = enc->e;
@@ -2027,6 +2035,64 @@ int b2w_debug_logits(b2w_model* h, b2w_encoded* enc, const int32_t* tokens, int3
           for (int i = i0; i < i1; ++i)
             memcpy(logits_out + ((size_t)(c0 + b) * n_tok + i) * V, tmp.data() + (size_t)(b * rpc + i - i0) * m->vpad, (size_t)V * 4);
       }
+    }
+  });
+}
+
+int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t P, int32_t n, int32_t K, int32_t n_steps,
+                          const int32_t* tokens, const int32_t* parents, float* logits_out) {
+  return guarded([&] {
+    B2W_CHECK(h && enc && enc->e && prompts && tokens && logits_out, "null argument");
+    Model* m = &h->m;
+    const b2w_config& c = m->cfg;
+    B2W_CHECK(enc->e->B == n, "one prompt per encoder output row is required");
+    B2W_CHECK(K >= 1 && K <= kMaxBeam, "rows per chunk must be in 1..16");
+    B2W_CHECK(n >= 1 && (int64_t)n * K <= kMaxRows, "chunks x rows per chunk must be in 1..80");
+    const int R = n * K, V = c.n_vocab, n_ctx = c.n_text_ctx;
+    B2W_CHECK(P >= 1 && n_steps >= 1 && P - 1 + n_steps <= n_ctx, "prompt length + steps exceed the text context");
+    for (size_t i = 0; i < (size_t)n * P; ++i) B2W_CHECK(prompts[i] >= 0 && prompts[i] < V, "prompt token id out of range");
+    for (size_t i = 0; i < (size_t)n_steps * R; ++i) B2W_CHECK(tokens[i] >= 0 && tokens[i] < V, "token id out of range");
+    if (parents)
+      for (size_t i = 0; i < (size_t)n_steps * R; ++i) B2W_CHECK(parents[i] >= 0 && parents[i] < K, "parent slot out of range");
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard g(m->device);
+    Step st = choose_step(m, n, K, false);
+    ensure_decoder_ws(m, n, K);
+    ensure_search_ws(m, n, K);
+    Encoded* e = enc->e;
+    ensure_cross_kv(m, e);
+    cudaStream_t s = m->stream;
+    const SearchBuffers& sb = m->sb;
+    B2W_CUDA(cudaMemsetAsync(sb.anc, 0, (size_t)2 * R * n_ctx, s));
+    if (P > 1) prefill(m, e, 0, n, prompts, P, K, -1, false);
+    b2w_gen_opts o;
+    b2w_gen_opts_default(&o);
+    o.beam_size = K;
+    o.max_length = P + n_steps;
+    bind_step(m, st, e, 0, prompts, P, search_params(m, prompts, n, K, P, -1, o));
+    // anc[r][j]: the slot that holds key j of row r.  Keys of the prompt sit in slot 0; relinked as search_update does.
+    std::vector<uint8_t> anc((size_t)R * n_ctx, 0), prev;
+    std::vector<RowInfo> rows(R);
+    for (int t = 0; t < n_steps; ++t) {
+      const int pos = P - 1 + t;
+      if (t > 0 && parents) {
+        prev = anc;
+        for (int r = 0; r < R; ++r) {
+          const int p = parents[(size_t)t * R + r], src = (r / K) * K + p;
+          memcpy(&anc[(size_t)r * n_ctx], &prev[(size_t)src * n_ctx], pos - 1);
+          anc[(size_t)r * n_ctx + pos - 1] = (uint8_t)p;
+        }
+      } else if (t > 0) {
+        for (int r = 0; r < R; ++r) anc[(size_t)r * n_ctx + pos - 1] = (uint8_t)(r % K);
+      }
+      for (int r = 0; r < R; ++r) rows[r] = RowInfo{r / K, r % K, pos, 0};
+      B2W_CUDA(cudaMemcpyAsync(sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, s));
+      B2W_CUDA(cudaMemcpyAsync(sb.tokens_in, tokens + (size_t)t * R, R * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+      B2W_CUDA(cudaMemcpyAsync(sb.anc + (size_t)(pos & 1) * R * n_ctx, anc.data(), anc.size(), cudaMemcpyHostToDevice, s));
+      launch_decoder(m, st);
+      B2W_CUDA(cudaMemcpy2DAsync(logits_out + (size_t)t * R * V, (size_t)V * 4, m->d_logits, (size_t)m->vpad * 4, (size_t)V * 4, R,
+                                 cudaMemcpyDeviceToHost, s));
+      B2W_CUDA(cudaStreamSynchronize(s));  // rows / anc are rewritten for the next step
     }
   });
 }

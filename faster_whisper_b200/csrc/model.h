@@ -101,7 +101,9 @@ struct Model {
   MelChunkDesc* e_chunks = nullptr;
   int* e_chunk_max = nullptr;
   std::map<int, EncPlan> enc_plans;
-  std::map<std::tuple<const void*, const void*, int, int>, GemmPlan> dec_plans;
+  // keyed by (weights, activations, rows, mode, row table, K cache, V cache, slots): the QKV epilogue's plan holds the last four,
+  // which change when the search or KV workspace is reallocated or the rows per chunk change
+  std::map<std::tuple<const void*, const void*, int, int, const void*, const void*, const void*, int>, GemmPlan> dec_plans;
 
   // decoder workspace
   int dw_rows = 0;

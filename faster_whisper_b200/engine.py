@@ -58,6 +58,7 @@ ABI_SYMBOLS = (
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
     "b2w_detect_language", "b2w_align", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
+    "b2w_debug_step_logits",
 )
 
 
@@ -117,6 +118,8 @@ def load_library():
                                        C.c_int32, C.c_void_p]
         lib.b2w_debug_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
         lib.b2w_debug_fetch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
+        lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]
         if lib.b2w_abi_version() != 1:
             raise RuntimeError("libb200whisper ABI version mismatch")
         _lib = lib
@@ -590,6 +593,29 @@ class Whisper:
         rep = self._replica_for(enc)
         with rep.lock:
             _check(rep._lib.b2w_debug_logits(rep.handle, enc._handle, _ptr(tokens), n, B, _ptr(out)))
+        return out
+
+    def debug_step_logits(self, enc: StorageView, prompts: np.ndarray, tokens: np.ndarray, parents: Optional[np.ndarray] = None) -> np.ndarray:
+        """Teacher-forced run of the decode-step path generate() would take for n chunks x K rows (tests only).
+
+        prompts [n, P]: positions 0..P-2 are prefilled.  tokens [n_steps, n, K]: step t feeds tokens[t, b, k] at position P-1+t.
+        parents [n_steps, n, K] (row 0 unused): the slot of the same chunk whose history the row continues, as after a beam
+        search's reordering; None keeps every slot on its own history.  Returns logits [n_steps, n, K, n_vocab]."""
+        prompts = np.ascontiguousarray(prompts, dtype=np.int32)
+        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+        n, P = prompts.shape
+        n_steps, tn, K = tokens.shape
+        if tn != n:
+            raise ValueError("tokens must be [n_steps, n_chunks, rows_per_chunk]")
+        if parents is not None:
+            parents = np.ascontiguousarray(parents, dtype=np.int32)
+            if parents.shape != tokens.shape:
+                raise ValueError("parents must have the shape of tokens")
+        out = np.empty((n_steps, n, K, self.dims.n_vocab), dtype=np.float32)
+        rep = self._replica_for(enc)
+        with rep.lock:
+            _check(rep._lib.b2w_debug_step_logits(rep.handle, enc._handle, _ptr(prompts), P, n, K, n_steps, _ptr(tokens), _ptr(parents),
+                                                  _ptr(out)))
         return out
 
 

@@ -172,6 +172,13 @@ int b2w_debug_gemv(int32_t device, int32_t impl, const float* x, const float* w,
 /* teacher-forced logits: run the decoder over tokens [batch, n] and return float32 [batch, n, n_vocab] */
 int b2w_debug_logits(b2w_model* m, b2w_encoded* e, const int32_t* tokens, int32_t n, int32_t batch,
                      float* logits_out);
+/* Run the model's decode-step path (the one generate() would choose for n chunks x K rows, or B2W_STEP's) for n_steps steps with
+ * forced inputs.  prompts [n][P]: positions 0..P-2 are prefilled into self-KV slot 0.  Step t feeds tokens[t][b*K+k] at position
+ * P-1+t as row (chunk b, slot k).  For t >= 1 the row continues the history of slot parents[t][b*K+k] of the same chunk as it
+ * stood after step t-1 (the relinking of the beam search); parents == NULL means every slot continues itself.
+ * logits_out [n_steps][n*K][n_vocab].  Every argument is checked before anything runs on the device. */
+int b2w_debug_step_logits(b2w_model* m, b2w_encoded* e, const int32_t* prompts, int32_t P, int32_t n, int32_t K,
+                          int32_t n_steps, const int32_t* tokens, const int32_t* parents, float* logits_out);
 
 /* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 raw QKV
  * sums [R][3d], 2 raw cross-q sums [R][d], 3 raw FFN hidden sums [R][4d], 4 attention output [R][d], 5 GELU(hidden) [R][4d],
