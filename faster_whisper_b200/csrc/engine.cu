@@ -835,12 +835,11 @@ static void ensure_cross_kv(Model* m, Encoded* e) {
 
 constexpr int kTcMinRows = 17;  // rows above which the decode GEMMs go through the wgmma path (activations reused from smem)
 
-// decode GEMM through the tensor-core GEMM: the plan (TMA maps and the epilogue's pointers) is cached per Model::dec_plans key
-static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
-  const auto key = std::make_tuple((const void*)a.W, (const void*)a.x, a.R, a.mode, (const void*)a.rows, (const void*)a.kcache,
-                                   (const void*)a.vcache, a.slots);
-  auto it = m->dec_plans.find(key);
-  if (it != m->dec_plans.end()) return it->second;
+// whether a decode GEMM goes through the tensor-core GEMM (else the skinny mma.sync kernel)
+static bool gv_uses_wgmma(const GvArgs& a) { return a.R >= kTcMinRows && a.K % 64 == 0 && a.N % 32 == 0; }
+
+// the tensor-core GEMM that computes a decode GEMM: the same outputs, 32-wide tiles where they give more CTAs
+static GemmArgs gv_gemm_args(const GvArgs& a) {
   GemmArgs g;
   g.A = a.x;
   g.a_batch = 1;
@@ -874,16 +873,29 @@ static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
     }
     case GV_F32: g.epilogue = EPI_F32; g.out = a.out_f; g.out_ld = a.ldo; break;
   }
-  return m->dec_plans.emplace(key, gemm_plan(g, m->num_sms)).first->second;
+  return g;
+}
+
+// decode GEMM through the tensor-core GEMM: the plan (TMA maps and the epilogue's pointers) is cached per Model::dec_plans key
+static const GemmPlan& dec_plan(Model* m, const GvArgs& a) {
+  const auto key = std::make_tuple((const void*)a.W, (const void*)a.x, a.R, a.mode, (const void*)a.rows, (const void*)a.kcache,
+                                   (const void*)a.vcache, a.slots);
+  auto it = m->dec_plans.find(key);
+  if (it != m->dec_plans.end()) return it->second;
+  return m->dec_plans.emplace(key, gemm_plan(gv_gemm_args(a), m->num_sms)).first->second;
+}
+
+// the wgmma route of a decode GEMM with plan `p` (gv_gemm_args(a)): the GEMM, then the next LayerNorm of a residual update
+static void gv_wgmma(const GemmPlan& p, const GvArgs& a, cudaStream_t s) {
+  gemm_run(p, s);
+  if (a.mode == GV_RESID_LN) layernorm_f32_f16(a.xres, a.ln_g, a.ln_b, a.xn_out, a.R, a.N, s);
 }
 
 static void gv(Model* m, GvArgs a) {
-  if (a.R >= kTcMinRows && a.K % 64 == 0 && a.N % 32 == 0) {
-    gemm_run(dec_plan(m, a), m->stream);
-    if (a.mode == GV_RESID_LN) layernorm_f32_f16(a.xres, a.ln_g, a.ln_b, a.xn_out, a.R, a.N, m->stream);
-    return;
-  }
-  skinny_gemm(a, m->stream);
+  if (gv_uses_wgmma(a))
+    gv_wgmma(dec_plan(m, a), a, m->stream);
+  else
+    skinny_gemm(a, m->stream);
 }
 
 static void bind_encoded(Model* m, const Encoded* e, int chunk0) {
@@ -1333,6 +1345,45 @@ struct b2w_model {
 struct b2w_encoded {
   Encoded* e;
 };
+
+// ---- helpers of the test hooks ----------------------------------------------------------------------------------------
+static_assert(B2W_EPI_F16 == EPI_F16 && B2W_EPI_GELU_F16 == EPI_GELU_F16 && B2W_EPI_RESID_F32 == EPI_RESID_F32 &&
+                  B2W_EPI_GELU_POS_F32 == EPI_GELU_POS_F32 && B2W_EPI_F16_XKV == EPI_F16_XKV && B2W_EPI_F32 == EPI_F32 &&
+                  B2W_EPI_QKV_CACHE == EPI_QKV_CACHE, "public epilogue ids");
+static_assert(B2W_GV_QKV == GV_QKV && B2W_GV_F16 == GV_F16 && B2W_GV_GELU_F16 == GV_GELU_F16 && B2W_GV_RESID_LN == GV_RESID_LN &&
+                  B2W_GV_F32 == GV_F32, "public decode GEMM modes");
+
+// Device copies of a test hook's host buffers, freed when the hook returns or throws.
+struct HookBufs {
+  std::vector<void*> ptrs;
+  ~HookBufs() {
+    for (void* p : ptrs) cudaFree(p);
+  }
+  // n_dev elements (at least n_host), zeroed, then the first n_host copied from `host` (nothing when it is NULL)
+  template <typename T>
+  T* put(const void* host, size_t n_host, size_t n_dev = 0) {
+    n_dev = std::max(n_dev, n_host);
+    T* p = dalloc<T>(n_dev);
+    ptrs.push_back(p);
+    B2W_CUDA(cudaMemset(p, 0, std::max<size_t>(n_dev, 1) * sizeof(T)));
+    if (host && n_host) B2W_CUDA(cudaMemcpy(p, host, n_host * sizeof(T), cudaMemcpyHostToDevice));
+    return p;
+  }
+};
+static void hook_get(void* host, const void* dev, size_t bytes) {
+  if (host) B2W_CUDA(cudaMemcpy(host, dev, bytes, cudaMemcpyDeviceToHost));
+}
+
+// rows x (chunk, slot, pos, -) must address entries of a [chunk][n_ctx][slots][d] cache of cache_elems halves
+static void check_row_table(const int32_t* rows, int R, int n_ctx, int slots, int d, int64_t cache_elems) {
+  B2W_CHECK(rows && n_ctx >= 1 && slots >= 1 && d >= 1, "row table and cache geometry");
+  for (int r = 0; r < R; ++r) {
+    const int32_t* ri = rows + 4 * r;
+    B2W_CHECK(ri[0] >= 0 && ri[1] >= 0 && ri[1] < slots && ri[2] >= 0 && ri[2] < n_ctx &&
+                  (((int64_t)ri[0] * n_ctx + ri[2]) * slots + ri[1] + 1) * d <= cache_elems,
+              "row table entry outside the cache");
+  }
+}
 
 extern "C" {
 
@@ -1885,40 +1936,93 @@ int b2w_counters_get(b2w_model* h, int64_t* launches, int64_t* decode_steps, dou
 }
 
 // ---- test hooks -------------------------------------------------------------------------------------------------------
-int b2w_debug_gemm(int32_t device, int32_t impl, const float* a, const float* w, const float* bias, int32_t M, int32_t N,
-                   int32_t K, int32_t gelu, float* c_out) {
+int b2w_debug_gemm(int32_t device, int32_t impl, b2w_gemm_desc* d) {
   return guarded([&] {
+    B2W_CHECK(d && d->a && d->w && d->out, "null argument");
+    B2W_CHECK(impl == 0 || impl == 1, "impl is 0 (wgmma) or 1 (SIMT reference)");
+    B2W_CHECK(d->taps >= 1 && d->taps <= 3, "1..3 taps");
+    B2W_CHECK(d->k_per_tap > 0 && d->k_per_tap % 64 == 0, "K per tap must be a multiple of 64");
+    B2W_CHECK(d->N > 0 && d->N % 32 == 0, "N must be a multiple of 32");
+    B2W_CHECK(d->a_batch >= 1 && d->a_rows >= 1 && d->a_cols >= 1 && d->rows >= 1, "empty GEMM");
+    B2W_CHECK(d->a_row_stride >= d->a_cols && d->a_row_stride % 8 == 0 && (d->a_batch == 1 || d->a_batch_stride % 8 == 0),
+              "A strides must be 16-byte multiples");
+    B2W_CHECK((d->a_batch - 1) * d->a_batch_stride + (d->a_rows - 1) * d->a_row_stride + d->a_cols <= d->a_elems,
+              "A exceeds its buffer");
+    for (int t = 0; t < d->taps; ++t) B2W_CHECK(d->tap_col[t] >= 0, "tap columns must be >= 0");
+    const int epi = d->epilogue;
+    B2W_CHECK(epi >= EPI_F16 && epi <= EPI_QKV_CACHE, "unknown epilogue");
+    const bool f16_out = epi == EPI_F16 || epi == EPI_GELU_F16 || epi == EPI_F16_XKV || epi == EPI_QKV_CACHE;
+    if (epi == EPI_F16_XKV) {
+      B2W_CHECK(d->xkv_heads >= 1 && d->xkv_d == 64 * d->xkv_heads && d->N % (2 * d->xkv_d) == 0,
+                "XKV: d = 64 x heads and N = layers x 2d");
+      B2W_CHECK(d->xkv_B == d->a_batch && d->xkv_T >= d->rows, "XKV: one output chunk per batch item and T >= rows");
+      B2W_CHECK((int64_t)d->N * d->xkv_B * d->xkv_T <= d->out_elems, "XKV output exceeds its buffer");
+    } else if (epi == EPI_QKV_CACHE) {
+      B2W_CHECK(d->a_batch == 1 && d->qkv_d > 0 && d->qkv_d % 32 == 0 && d->N == 3 * d->qkv_d, "QKV: one batch item and N = 3d");
+      B2W_CHECK((int64_t)d->rows * d->qkv_d <= d->out_elems, "q output exceeds its buffer");
+      B2W_CHECK(d->kcache && d->vcache, "QKV: both caches");
+      check_row_table(d->rowinfo, d->rows, d->n_ctx, d->slots, d->qkv_d, d->cache_elems);
+    } else {
+      const int vec = f16_out ? 8 : 4;  // 16-byte vector stores
+      B2W_CHECK(d->out_ld >= d->N && d->out_ld % vec == 0 && (d->a_batch == 1 || d->out_batch_stride % vec == 0),
+                "output strides must be 16-byte multiples");
+      B2W_CHECK((d->a_batch - 1) * d->out_batch_stride + (int64_t)(d->rows - 1) * d->out_ld + d->N <= d->out_elems,
+                "output exceeds its buffer");
+      B2W_CHECK(epi != EPI_GELU_POS_F32 || d->pos, "GELU_POS needs pos");
+    }
     require_hopper(device);
     DeviceGuard g(device);
-    cudaDeviceProp prop;
-    B2W_CUDA(cudaGetDeviceProperties(&prop, device));
-    float *da = dalloc<float>((size_t)M * K), *dw = dalloc<float>((size_t)N * K), *db = dalloc<float>(N);
-    __half *ha = dalloc<__half>((size_t)M * K), *hw = dalloc<__half>((size_t)N * K), *hc = dalloc<__half>((size_t)M * N);
-    float* dc = dalloc<float>((size_t)M * N);
-    B2W_CUDA(cudaMemcpy(da, a, (size_t)M * K * 4, cudaMemcpyHostToDevice));
-    B2W_CUDA(cudaMemcpy(dw, w, (size_t)N * K * 4, cudaMemcpyHostToDevice));
-    if (bias) B2W_CUDA(cudaMemcpy(db, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
-    convert_f32_f16(da, ha, (int64_t)M * K, 0);
-    convert_f32_f16(dw, hw, (int64_t)N * K, 0);
+    HookBufs hb;
+    const int64_t K = (int64_t)d->taps * d->k_per_tap;
+    const size_t out_bytes = (size_t)d->out_elems * (f16_out ? 2 : 4);
     GemmArgs ga;
-    ga.A = ha; ga.a_batch = 1; ga.a_rows = M; ga.a_cols = K; ga.a_row_stride = K; ga.k_per_tap = K;
-    ga.W = hw; ga.N = N; ga.rows = M; ga.bias = bias ? db : nullptr;
-    if (gelu) {
-      ga.out = hc; ga.out_ld = N; ga.epilogue = EPI_GELU_F16;
-    } else {
-      ga.out = dc; ga.out_ld = N; ga.epilogue = EPI_F32;
+    ga.A = hb.put<__half>(d->a, d->a_elems);
+    ga.a_batch = d->a_batch; ga.a_rows = d->a_rows; ga.a_cols = d->a_cols;
+    ga.a_row_stride = d->a_row_stride; ga.a_batch_stride = d->a_batch_stride;
+    ga.taps = d->taps;
+    for (int t = 0; t < 3; ++t) {
+      ga.tap_row[t] = d->tap_row[t];
+      ga.tap_col[t] = d->tap_col[t];
     }
+    ga.k_per_tap = d->k_per_tap;
+    ga.W = hb.put<__half>(d->w, (size_t)d->N * K);
+    ga.N = d->N;
+    ga.rows = d->rows;
+    ga.bias = d->bias ? hb.put<float>(d->bias, d->N) : nullptr;
+    ga.out = hb.put<uint8_t>(d->out, out_bytes);
+    ga.out_ld = d->out_ld;
+    ga.out_batch_stride = d->out_batch_stride;
+    if (epi == EPI_RESID_F32) ga.resid = reinterpret_cast<const float*>(ga.out);
+    if (epi == EPI_GELU_POS_F32) ga.pos = hb.put<float>(d->pos, (size_t)d->rows * d->N);
+    ga.xkv_d = d->xkv_d; ga.xkv_heads = d->xkv_heads; ga.xkv_T = d->xkv_T; ga.xkv_B = d->xkv_B;
+    if (epi == EPI_QKV_CACHE) {
+      ga.rowinfo = reinterpret_cast<const int4*>(hb.put<int32_t>(d->rowinfo, (size_t)4 * d->rows));
+      ga.kcache = hb.put<__half>(d->kcache, d->cache_elems);
+      ga.vcache = hb.put<__half>(d->vcache, d->cache_elems);
+      ga.qkv_d = d->qkv_d; ga.n_ctx = d->n_ctx; ga.slots = d->slots;
+    }
+    ga.epilogue = epi;
+    ga.narrow_tiles = d->narrow_tiles != 0;
+    d->block_n_out = d->grid_out = 0;
     if (impl == 0) {
       gemm_configure();  // per-device kernel attributes (build_model does this for real models)
+      cudaDeviceProp prop;
+      B2W_CUDA(cudaGetDeviceProperties(&prop, device));
       GemmPlan p = gemm_plan(ga, prop.multiProcessorCount);
+      // fewer persistent CTAs than the plan's: the same tiles, several per CTA
+      if (d->max_ctas > 0) p.grid = std::min(p.grid, (int)d->max_ctas);
+      d->block_n_out = p.block_n;
+      d->grid_out = p.grid;
       gemm_run(p, 0);
     } else {
       gemm_ref_run(ga, 0);
     }
-    if (gelu) convert_f16_f32(hc, dc, (int64_t)M * N, 0);
     B2W_CUDA(cudaDeviceSynchronize());
-    B2W_CUDA(cudaMemcpy(c_out, dc, (size_t)M * N * 4, cudaMemcpyDeviceToHost));
-    cudaFree(da); cudaFree(dw); cudaFree(db); cudaFree(ha); cudaFree(hw); cudaFree(hc); cudaFree(dc);
+    hook_get(d->out, ga.out, out_bytes);
+    if (epi == EPI_QKV_CACHE) {
+      hook_get(d->kcache, ga.kcache, (size_t)d->cache_elems * 2);
+      hook_get(d->vcache, ga.vcache, (size_t)d->cache_elems * 2);
+    }
   });
 }
 
@@ -1944,34 +2048,84 @@ int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t 
   });
 }
 
-int b2w_debug_gemv(int32_t device, int32_t impl, const float* x, const float* w, const float* bias, int32_t R, int32_t N,
-                   int32_t K, float* y_out) {
+int b2w_debug_gemv(int32_t device, int32_t impl, b2w_gemv_desc* d) {
   return guarded([&] {
+    B2W_CHECK(d && d->x && d->w, "null argument");
+    B2W_CHECK(d->mode >= GV_QKV && d->mode <= GV_F32, "unknown mode");
+    B2W_CHECK(impl == 0 || (impl == 1 && d->mode == GV_F32 && d->ldo == d->N), "impl 1 (reference) computes mode F32 with ldo = N");
+    B2W_CHECK(d->route == 0 || d->route == 1, "route is 0 (skinny kernel) or 1 (the decoder's choice)");
+    B2W_CHECK(d->R >= 1 && d->R <= kMaxRows, "1..80 rows");
+    B2W_CHECK(d->N >= 1 && d->K >= 32 && d->K % 32 == 0, "K must be a multiple of 32");
+    const int R = d->R, N = d->N, K = d->K;
+    switch (d->mode) {
+      case GV_QKV:
+        B2W_CHECK(d->d > 0 && d->d % 32 == 0 && N == 3 * d->d, "QKV: N = 3d");
+        B2W_CHECK(d->out && (int64_t)R * d->d <= d->out_elems, "q output exceeds its buffer");
+        B2W_CHECK(d->kcache && d->vcache, "QKV: both caches");
+        check_row_table(d->rows, R, d->n_ctx, d->slots, d->d, d->cache_elems);
+        break;
+      case GV_F16:
+      case GV_GELU_F16: B2W_CHECK(d->out && (int64_t)R * N <= d->out_elems, "output exceeds its buffer"); break;
+      case GV_RESID_LN:
+        B2W_CHECK(d->xres && d->xn && N % 4 == 0 && N <= 1280, "RESID_LN: xres and xn, N a multiple of 4 up to 1280");
+        B2W_CHECK((d->ln_g == nullptr) == (d->ln_b == nullptr), "LayerNorm gamma and beta come together");
+        break;
+      case GV_F32:
+        B2W_CHECK(d->out && d->ldo >= N && d->ldo % 4 == 0 && (int64_t)(R - 1) * d->ldo + N <= d->out_elems, "output exceeds its buffer");
+        break;
+    }
     require_hopper(device);
     DeviceGuard g(device);
-    const int Np = ceil_div(N, 16) * 16, Rp = ceil_div(R, 8) * 8;
-    float *dx = dalloc<float>((size_t)Rp * K), *dw = dalloc<float>((size_t)Np * K), *db = dalloc<float>(Np), *dy = dalloc<float>((size_t)R * Np);
-    __half *hx = dalloc<__half>((size_t)Rp * K), *hw = dalloc<__half>((size_t)Np * K);
-    B2W_CUDA(cudaMemset(dx, 0, (size_t)Rp * K * 4));
-    B2W_CUDA(cudaMemset(dw, 0, (size_t)Np * K * 4));
-    B2W_CUDA(cudaMemset(db, 0, (size_t)Np * 4));
-    B2W_CUDA(cudaMemcpy(dx, x, (size_t)R * K * 4, cudaMemcpyHostToDevice));
-    B2W_CUDA(cudaMemcpy(dw, w, (size_t)N * K * 4, cudaMemcpyHostToDevice));
-    if (bias) B2W_CUDA(cudaMemcpy(db, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
-    convert_f32_f16(dx, hx, (int64_t)Rp * K, 0);
-    convert_f32_f16(dw, hw, (int64_t)Np * K, 0);
-    if (impl == 0) {
-      GvArgs a;
-      a.x = hx; a.W = hw; a.bias = bias ? db : nullptr; a.R = R; a.N = Np; a.K = K; a.mode = GV_F32; a.out_f = dy; a.ldo = Np;
-      skinny_gemm(a, 0);
+    HookBufs hb;
+    // zero-padded like the decoder's workspaces: the skinny kernel reads activations in 8-row groups up to kMaxRows rows and
+    // weights in 16-row groups
+    const int Np = ceil_div(N, 16) * 16;
+    const size_t out_bytes = d->out ? (size_t)d->out_elems * (d->mode == GV_F32 ? 4 : 2) : 0;
+    GvArgs a;
+    a.x = hb.put<__half>(d->x, (size_t)R * K, (size_t)kMaxRows * K);
+    a.W = hb.put<__half>(d->w, (size_t)N * K, (size_t)Np * K);
+    a.bias = d->bias ? hb.put<float>(d->bias, N) : nullptr;
+    a.R = R; a.N = N; a.K = K; a.mode = d->mode;
+    void* out = d->out ? hb.put<uint8_t>(d->out, out_bytes) : nullptr;
+    a.out_h = reinterpret_cast<__half*>(out);
+    a.out_f = reinterpret_cast<float*>(out);
+    a.ldo = d->ldo;
+    if (d->mode == GV_QKV) {
+      a.rows = reinterpret_cast<const RowInfo*>(hb.put<int32_t>(d->rows, (size_t)4 * R));
+      a.kcache = hb.put<__half>(d->kcache, d->cache_elems);
+      a.vcache = hb.put<__half>(d->vcache, d->cache_elems);
+      a.d = d->d; a.n_ctx = d->n_ctx; a.slots = d->slots;
+    }
+    if (d->mode == GV_RESID_LN) {
+      a.xres = hb.put<float>(d->xres, (size_t)R * N);
+      a.ln_g = d->ln_g ? hb.put<float>(d->ln_g, N) : nullptr;
+      a.ln_b = d->ln_b ? hb.put<float>(d->ln_b, N) : nullptr;
+      a.xn_out = hb.put<__half>(d->xn, (size_t)R * N);
+      a.counter = hb.put<int>(nullptr, 1);
+    }
+    d->path_out = 0;
+    if (impl == 1) {
+      skinny_ref(a.x, a.W, a.bias, a.out_f, R, N, K, 0);
+    } else if (d->route == 1 && gv_uses_wgmma(a)) {
+      // what gv() runs, with a plan built here rather than cached in a model
+      gemm_configure();
+      cudaDeviceProp prop;
+      B2W_CUDA(cudaGetDeviceProperties(&prop, device));
+      gv_wgmma(gemm_plan(gv_gemm_args(a), prop.multiProcessorCount), a, 0);
+      d->path_out = 1;
     } else {
-      skinny_ref(hx, hw, bias ? db : nullptr, dy, R, Np, K, 0);
+      skinny_gemm(a, 0);
     }
     B2W_CUDA(cudaDeviceSynchronize());
-    std::vector<float> tmp((size_t)R * Np);
-    B2W_CUDA(cudaMemcpy(tmp.data(), dy, tmp.size() * 4, cudaMemcpyDeviceToHost));
-    for (int r = 0; r < R; ++r) memcpy(y_out + (size_t)r * N, tmp.data() + (size_t)r * Np, (size_t)N * 4);
-    cudaFree(dx); cudaFree(dw); cudaFree(db); cudaFree(dy); cudaFree(hx); cudaFree(hw);
+    hook_get(d->out, out, out_bytes);
+    if (d->mode == GV_QKV) {
+      hook_get(d->kcache, a.kcache, (size_t)d->cache_elems * 2);
+      hook_get(d->vcache, a.vcache, (size_t)d->cache_elems * 2);
+    }
+    if (d->mode == GV_RESID_LN) {
+      hook_get(d->xres, a.xres, (size_t)R * N * 4);
+      hook_get(d->xn, a.xn_out, (size_t)R * N * 2);
+    }
   });
 }
 

@@ -51,6 +51,35 @@ class _GenOpts(C.Structure):
     ]
 
 
+class _GemmDesc(C.Structure):  # b2w_gemm_desc
+    _fields_ = [
+        ("a", C.c_void_p), ("a_elems", C.c_int64), ("a_batch", C.c_int32), ("a_rows", C.c_int32), ("a_cols", C.c_int32),
+        ("a_row_stride", C.c_int64), ("a_batch_stride", C.c_int64), ("taps", C.c_int32), ("tap_row", C.c_int32 * 3),
+        ("tap_col", C.c_int32 * 3), ("k_per_tap", C.c_int32), ("w", C.c_void_p), ("bias", C.c_void_p), ("N", C.c_int32),
+        ("rows", C.c_int32), ("epilogue", C.c_int32), ("narrow_tiles", C.c_int32), ("out", C.c_void_p), ("out_elems", C.c_int64),
+        ("out_ld", C.c_int64), ("out_batch_stride", C.c_int64), ("pos", C.c_void_p), ("xkv_d", C.c_int32), ("xkv_heads", C.c_int32),
+        ("xkv_T", C.c_int32), ("xkv_B", C.c_int32), ("rowinfo", C.c_void_p), ("kcache", C.c_void_p), ("vcache", C.c_void_p),
+        ("cache_elems", C.c_int64), ("qkv_d", C.c_int32), ("n_ctx", C.c_int32), ("slots", C.c_int32), ("max_ctas", C.c_int32),
+        ("block_n_out", C.c_int32), ("grid_out", C.c_int32),
+    ]
+
+
+class _GemvDesc(C.Structure):  # b2w_gemv_desc
+    _fields_ = [
+        ("x", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("R", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+        ("mode", C.c_int32), ("route", C.c_int32), ("rows", C.c_void_p), ("kcache", C.c_void_p), ("vcache", C.c_void_p),
+        ("cache_elems", C.c_int64), ("d", C.c_int32), ("n_ctx", C.c_int32), ("slots", C.c_int32), ("out", C.c_void_p),
+        ("out_elems", C.c_int64), ("ldo", C.c_int64), ("xres", C.c_void_p), ("ln_g", C.c_void_p), ("ln_b", C.c_void_p),
+        ("xn", C.c_void_p), ("path_out", C.c_int32),
+    ]
+
+
+# dense GEMM epilogues (include/b200whisper.h B2W_EPI_*) and decode GEMM modes (B2W_GV_*)
+EPI_F16, EPI_GELU_F16, EPI_RESID_F32, EPI_GELU_POS_F32, EPI_F16_XKV, EPI_F32, EPI_QKV_CACHE = range(7)
+EPI_F16_OUT = (EPI_F16, EPI_GELU_F16, EPI_F16_XKV, EPI_QKV_CACHE)
+GV_QKV, GV_F16, GV_GELU_F16, GV_RESID_LN, GV_F32 = range(5)
+
+
 # every symbol include/b200whisper.h declares (checked by tests/test_abi.py)
 ABI_SYMBOLS = (
     "b2w_last_error", "b2w_abi_version", "b2w_device_count", "b2w_model_create", "b2w_model_destroy",
@@ -111,11 +140,9 @@ def load_library():
         lib.b2w_span_begin.argtypes = [C.c_void_p]
         lib.b2w_span_end.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         lib.b2w_counters_get.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
-        lib.b2w_debug_gemm.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
-                                       C.c_int32, C.c_int32, C.c_void_p]
+        lib.b2w_debug_gemm.argtypes = [C.c_int32, C.c_int32, C.POINTER(_GemmDesc)]
         lib.b2w_debug_attention.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-        lib.b2w_debug_gemv.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
-                                       C.c_int32, C.c_void_p]
+        lib.b2w_debug_gemv.argtypes = [C.c_int32, C.c_int32, C.POINTER(_GemvDesc)]
         lib.b2w_debug_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
         lib.b2w_debug_fetch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
         lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
@@ -633,14 +660,64 @@ class models:  # namespace shim so `ctranslate2.models.Whisper` style access wor
     WhisperGenerationResult = WhisperGenerationResult
 
 
-def debug_gemm(a: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, gelu: bool = False, device: int = 0):
+def _buf(x: Optional[np.ndarray], dtype, name: str) -> Optional[np.ndarray]:
+    """A host buffer the hooks read or update in place: it must already have the dtype and be C-contiguous."""
+    if x is None:
+        return None
+    if x.dtype != dtype or not x.flags["C_CONTIGUOUS"]:
+        raise ValueError(f"{name} must be a C-contiguous {np.dtype(dtype).name} array")
+    return x
+
+
+def debug_gemm_desc(a: np.ndarray, w: np.ndarray, out: np.ndarray, *, epilogue: int, rows: int, a_batch: int = 1,
+                    a_rows: Optional[int] = None, a_cols: Optional[int] = None, a_row_stride: Optional[int] = None,
+                    a_batch_stride: int = 0, tap_row: Sequence[int] = (0,), tap_col: Sequence[int] = (0,),
+                    bias: Optional[np.ndarray] = None, out_ld: Optional[int] = None, out_batch_stride: int = 0,
+                    narrow_tiles: bool = False, pos: Optional[np.ndarray] = None, xkv: Tuple[int, int, int, int] = (0, 0, 0, 0),
+                    rowinfo: Optional[np.ndarray] = None, kcache: Optional[np.ndarray] = None, vcache: Optional[np.ndarray] = None,
+                    qkv_d: int = 0, n_ctx: int = 0, slots: int = 0, max_ctas: int = 0, impl: int = 0, device: int = 0) -> Tuple[int, int]:
+    """One dense GEMM as the engine states it (b2w_gemm_desc; tests only).  a: float16 buffer of A, w: float16 [N, taps*k_per_tap],
+    out (float16 or float32 by epilogue) and the caches are updated in place; xkv = (d, heads, T, B).  Returns the (tile width,
+    grid) the plan chose (0, 0 for the reference)."""
     lib = load_library()
-    a = np.ascontiguousarray(a, np.float32)
-    w = np.ascontiguousarray(w, np.float32)
-    b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-    out = np.empty((a.shape[0], w.shape[0]), np.float32)
-    _check(lib.b2w_debug_gemm(device, impl, _ptr(a), _ptr(w), _ptr(b), a.shape[0], w.shape[0], a.shape[1], int(gelu), _ptr(out)))
-    return out
+    a, w = _buf(a, np.float16, "a"), _buf(w, np.float16, "w")
+    out = _buf(out, np.float16 if epilogue in EPI_F16_OUT else np.float32, "out")
+    bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
+    pos = None if pos is None else np.ascontiguousarray(pos, np.float32)
+    rowinfo = None if rowinfo is None else np.ascontiguousarray(rowinfo, np.int32)
+    kcache, vcache = _buf(kcache, np.float16, "kcache"), _buf(vcache, np.float16, "vcache")
+    if len(tap_row) != len(tap_col) or not 1 <= len(tap_row) <= 3:
+        raise ValueError("1..3 taps, one row and one column offset each")
+    N, K = w.shape
+    taps = len(tap_row)
+    d = _GemmDesc()
+    d.a, d.a_elems, d.a_batch = _ptr(a), a.size, a_batch
+    d.a_rows = rows if a_rows is None else a_rows
+    d.a_cols = K // taps if a_cols is None else a_cols
+    d.a_row_stride = d.a_cols if a_row_stride is None else a_row_stride
+    d.a_batch_stride = a_batch_stride
+    d.taps, d.k_per_tap = taps, K // taps
+    d.tap_row[:] = list(tap_row) + [0] * (3 - taps)
+    d.tap_col[:] = list(tap_col) + [0] * (3 - taps)
+    d.w, d.bias, d.N, d.rows, d.epilogue, d.narrow_tiles = _ptr(w), _ptr(bias), N, rows, epilogue, int(narrow_tiles)
+    d.out, d.out_elems = _ptr(out), out.size
+    d.out_ld = N if out_ld is None else out_ld
+    d.out_batch_stride, d.pos = out_batch_stride, _ptr(pos)
+    d.xkv_d, d.xkv_heads, d.xkv_T, d.xkv_B = xkv
+    d.rowinfo, d.kcache, d.vcache = _ptr(rowinfo), _ptr(kcache), _ptr(vcache)
+    d.cache_elems = 0 if kcache is None else min(kcache.size, vcache.size if vcache is not None else 0)
+    d.qkv_d, d.n_ctx, d.slots, d.max_ctas = qkv_d, n_ctx, slots, max_ctas
+    _check(lib.b2w_debug_gemm(device, impl, C.byref(d)))
+    return d.block_n_out, d.grid_out
+
+
+def debug_gemm(a: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, gelu: bool = False, device: int = 0):
+    """C = A W^T + bias (or fp16 GELU of it) for float32 A [M, K], W [N, K] rounded to fp16; float32 result."""
+    a16 = np.ascontiguousarray(a, np.float32).astype(np.float16)
+    w16 = np.ascontiguousarray(w, np.float32).astype(np.float16)
+    out = np.zeros((a16.shape[0], w16.shape[0]), np.float16 if gelu else np.float32)
+    debug_gemm_desc(a16, w16, out, epilogue=EPI_GELU_F16 if gelu else EPI_F32, rows=a16.shape[0], bias=bias, impl=impl, device=device)
+    return out.astype(np.float32)
 
 
 def debug_attention(qkv: np.ndarray, heads: int, impl: int = 0, device: int = 0):
@@ -652,11 +729,39 @@ def debug_attention(qkv: np.ndarray, heads: int, impl: int = 0, device: int = 0)
     return out
 
 
-def debug_gemv(x: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, device: int = 0):
+def debug_gemv_desc(x: np.ndarray, w: np.ndarray, *, mode: int, bias: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
+                    ldo: int = 0, rows: Optional[np.ndarray] = None, kcache: Optional[np.ndarray] = None,
+                    vcache: Optional[np.ndarray] = None, d: int = 0, n_ctx: int = 0, slots: int = 0, xres: Optional[np.ndarray] = None,
+                    ln_g: Optional[np.ndarray] = None, ln_b: Optional[np.ndarray] = None, xn: Optional[np.ndarray] = None,
+                    route: int = 1, impl: int = 0, device: int = 0) -> int:
+    """One decoder GEMM of R = x.shape[0] <= 80 rows (b2w_gemv_desc; tests only).  x: float16 [R, K], w: float16 [N, K]; out
+    (float32 for GV_F32, else float16), the caches, xres (float32) and xn (float16) are updated in place.  route 1 runs what the
+    decoder runs for this shape, route 0 the skinny kernel.  Returns the path that ran: 0 skinny, 1 wgmma."""
     lib = load_library()
-    x = np.ascontiguousarray(x, np.float32)
-    w = np.ascontiguousarray(w, np.float32)
-    b = None if bias is None else np.ascontiguousarray(bias, np.float32)
-    out = np.empty((x.shape[0], w.shape[0]), np.float32)
-    _check(lib.b2w_debug_gemv(device, impl, _ptr(x), _ptr(w), _ptr(b), x.shape[0], w.shape[0], x.shape[1], _ptr(out)))
+    x, w = _buf(x, np.float16, "x"), _buf(w, np.float16, "w")
+    out = _buf(out, np.float32 if mode == GV_F32 else np.float16, "out")
+    bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
+    rows = None if rows is None else np.ascontiguousarray(rows, np.int32)
+    kcache, vcache = _buf(kcache, np.float16, "kcache"), _buf(vcache, np.float16, "vcache")
+    xres, xn = _buf(xres, np.float32, "xres"), _buf(xn, np.float16, "xn")
+    ln_g = None if ln_g is None else np.ascontiguousarray(ln_g, np.float32)
+    ln_b = None if ln_b is None else np.ascontiguousarray(ln_b, np.float32)
+    R, K = x.shape
+    desc = _GemvDesc()
+    desc.x, desc.w, desc.bias, desc.R, desc.N, desc.K, desc.mode, desc.route = _ptr(x), _ptr(w), _ptr(bias), R, w.shape[0], K, mode, route
+    desc.rows, desc.kcache, desc.vcache = _ptr(rows), _ptr(kcache), _ptr(vcache)
+    desc.cache_elems = 0 if kcache is None else min(kcache.size, vcache.size if vcache is not None else 0)
+    desc.d, desc.n_ctx, desc.slots = d, n_ctx, slots
+    desc.out, desc.out_elems, desc.ldo = _ptr(out), 0 if out is None else out.size, ldo
+    desc.xres, desc.ln_g, desc.ln_b, desc.xn = _ptr(xres), _ptr(ln_g), _ptr(ln_b), _ptr(xn)
+    _check(lib.b2w_debug_gemv(device, impl, C.byref(desc)))
+    return desc.path_out
+
+
+def debug_gemv(x: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, device: int = 0):
+    """y = x W^T + bias through the skinny kernel (impl 0) or its reference (impl 1), float32 x [R, K], W [N, K] rounded to fp16."""
+    x16 = np.ascontiguousarray(x, np.float32).astype(np.float16)
+    w16 = np.ascontiguousarray(w, np.float32).astype(np.float16)
+    out = np.zeros((x16.shape[0], w16.shape[0]), np.float32)
+    debug_gemv_desc(x16, w16, mode=GV_F32, bias=bias, out=out, ldo=w16.shape[0], route=0, impl=impl, device=device)
     return out

@@ -160,15 +160,78 @@ int b2w_span_end(b2w_model* m, double* ms_out);
 int b2w_counters_get(b2w_model* m, int64_t* launches, int64_t* decode_steps, double* decode_alg_bytes);
 
 /* ---- test hooks (used by tests/ only) ----------------------------------------------------------- */
-/* C = epilogue(A[M,K] * W[N,K]^T + bias) through the wgmma (impl=0) or reference SIMT (impl=1) GEMM. */
-int b2w_debug_gemm(int32_t device, int32_t impl, const float* a, const float* w, const float* bias,
-                   int32_t M, int32_t N, int32_t K, int32_t gelu, float* c_out);
+/* Epilogues of the dense GEMM (csrc/engine.h Epilogue). */
+enum { B2W_EPI_F16 = 0, B2W_EPI_GELU_F16 = 1, B2W_EPI_RESID_F32 = 2, B2W_EPI_GELU_POS_F32 = 3, B2W_EPI_F16_XKV = 4,
+       B2W_EPI_F32 = 5, B2W_EPI_QKV_CACHE = 6 };
+
+/* One dense GEMM as the engine states it (csrc/engine.h GemmArgs), with host buffers.  fp16 buffers are IEEE half bit
+ * patterns.  Output buffers are in/out: they are copied to the device, run, and copied back whole, so elements the kernel must
+ * not write keep whatever the caller put there. */
+typedef struct b2w_gemm_desc {
+  /* A: fp16 [a_batch][a_rows][a_cols] at the given element strides inside a host buffer of a_elems halves; K index k of tap t
+   * reads element (row + tap_row[t], tap_col[t] + k), zero outside the a_rows x a_cols box */
+  const uint16_t* a;
+  int64_t a_elems;
+  int32_t a_batch, a_rows, a_cols;
+  int64_t a_row_stride, a_batch_stride;
+  int32_t taps, tap_row[3], tap_col[3], k_per_tap; /* k_per_tap: multiple of 64 */
+  const uint16_t* w;                               /* fp16 [N][taps * k_per_tap] */
+  const float* bias;                               /* [N] or NULL */
+  int32_t N, rows, epilogue, narrow_tiles;         /* N: multiple of 32; rows per batch item */
+  /* out: fp16 (F16, GELU_F16, F16_XKV, QKV_CACHE) or float32 (RESID_F32, GELU_POS_F32, F32), out_elems elements;
+   * element (b, row, n) at b * out_batch_stride + row * out_ld + n.  RESID_F32 adds to out in place, as the engine does. */
+  void* out;
+  int64_t out_elems, out_ld, out_batch_stride;
+  const float* pos;                                /* GELU_POS_F32: [rows][N] */
+  int32_t xkv_d, xkv_heads, xkv_T, xkv_B;          /* F16_XKV: out is [N / (2 xkv_d)][2][xkv_B][xkv_heads][xkv_T][64] */
+  /* QKV_CACHE (a_batch = 1, N = 3 qkv_d): q -> out [rows][qkv_d]; k, v -> kcache / vcache [chunk][n_ctx][slots][qkv_d] at the
+   * (chunk, slot, pos) of rowinfo [rows][4] (the fourth int is unused); both caches hold cache_elems halves */
+  const int32_t* rowinfo;
+  uint16_t* kcache;
+  uint16_t* vcache;
+  int64_t cache_elems;
+  int32_t qkv_d, n_ctx, slots;
+  int32_t max_ctas;            /* > 0: at most this many persistent CTAs (tests: several tiles per CTA); 0: one per SM */
+  int32_t block_n_out, grid_out; /* written: the tile width and grid the plan chose (impl 0) */
+} b2w_gemm_desc;
+
+/* Run one described GEMM through the wgmma kernel (impl=0) or the plain SIMT reference of the same contract (impl=1).  Every
+ * argument (shapes, strides, buffer extents, row table) is checked before anything runs on the device. */
+int b2w_debug_gemm(int32_t device, int32_t impl, b2w_gemm_desc* desc);
 /* softmax(QK^T/8)V for [B,T,H*64] fp16-rounded inputs through the wgmma (0) or reference (1) kernel. */
 int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t B, int32_t T, int32_t H,
                         float* out);
-/* one decode-style skinny GEMM y[R,N] = x[R,K] W[N,K]^T + b through the mma.sync (0) or reference (1) path */
-int b2w_debug_gemv(int32_t device, int32_t impl, const float* x, const float* w, const float* bias,
-                   int32_t R, int32_t N, int32_t K, float* y_out);
+/* Modes of the decode GEMM (csrc/decode.h GvMode). */
+enum { B2W_GV_QKV = 0, B2W_GV_F16 = 1, B2W_GV_GELU_F16 = 2, B2W_GV_RESID_LN = 3, B2W_GV_F32 = 4 };
+
+/* One decoder GEMM y = x[R,K] W[N,K]^T + bias of R <= 80 rows, with the epilogue of `mode`.  Output buffers are in/out as in
+ * b2w_gemm_desc. */
+typedef struct b2w_gemv_desc {
+  const uint16_t* x;  /* fp16 [R][K] */
+  const uint16_t* w;  /* fp16 [N][K] */
+  const float* bias;  /* [N] or NULL */
+  int32_t R, N, K, mode;
+  int32_t route;      /* 0: the skinny mma.sync kernel; 1: the path the decoder takes for this shape */
+  /* QKV (N = 3 d): q -> out [R][d]; k, v -> kcache / vcache [chunk][n_ctx][slots][d] at rows[r] = (chunk, slot, pos, -) */
+  const int32_t* rows;
+  uint16_t* kcache;
+  uint16_t* vcache;
+  int64_t cache_elems;
+  int32_t d, n_ctx, slots;
+  /* F16, GELU_F16: fp16 [R][N]; F32: float32 [R][ldo]; QKV: fp16 [R][d]; out_elems elements */
+  void* out;
+  int64_t out_elems, ldo;
+  /* RESID_LN (N <= 1280): xres [R][N] += y, then xn [R][N] (fp16) = LayerNorm(xres) * ln_g + ln_b (NULL: no affine) */
+  float* xres;
+  const float* ln_g;
+  const float* ln_b;
+  uint16_t* xn;
+  int32_t path_out;   /* written: 0 the skinny kernel ran, 1 the wgmma GEMM ran */
+} b2w_gemv_desc;
+
+/* Run one described decoder GEMM (impl=0), or with impl=1 and mode F32 the one-thread-per-output reference.  Every argument is
+ * checked before anything runs on the device. */
+int b2w_debug_gemv(int32_t device, int32_t impl, b2w_gemv_desc* desc);
 /* teacher-forced logits: run the decoder over tokens [batch, n] and return float32 [batch, n, n_vocab] */
 int b2w_debug_logits(b2w_model* m, b2w_encoded* e, const int32_t* tokens, int32_t n, int32_t batch,
                      float* logits_out);

@@ -38,6 +38,25 @@ def test_struct_layout_matches_header():
     assert o.debug_fake_logits == 0 and o.seed == 0 and o.n_suppress_tokens == 0
 
 
+def test_gemm_hooks_check_arguments_before_the_device():
+    """Bad GEMM descriptors are refused (ValueError) before anything touches a device, GPU or not."""
+    a, out = np.zeros(64 * 64, np.float16), np.zeros(64 * 128, np.float32)
+    w = np.zeros((128, 64), np.float16)
+    with pytest.raises(ValueError, match="N must be a multiple of 32"):
+        engine.debug_gemm_desc(a, np.zeros((48, 64), np.float16), out, epilogue=engine.EPI_F32, rows=64)
+    with pytest.raises(ValueError, match="K per tap"):
+        engine.debug_gemm_desc(a, np.zeros((128, 96), np.float16), out, epilogue=engine.EPI_F32, rows=64, a_cols=96)
+    with pytest.raises(ValueError, match="exceeds its buffer"):
+        engine.debug_gemm_desc(a, w, out, epilogue=engine.EPI_F32, rows=65, a_rows=64)
+    kc = np.zeros((1, 4, 2, 64), np.float16)
+    rows = np.array([[0, 1, 3, 0]] * 63 + [[0, 2, 0, 0]], np.int32)  # slot 2 of 2
+    with pytest.raises(ValueError, match="row table"):
+        engine.debug_gemm_desc(a, np.zeros((192, 64), np.float16), np.zeros(64 * 64, np.float16), epilogue=engine.EPI_QKV_CACHE, rows=64,
+                               rowinfo=rows, kcache=kc, vcache=kc.copy(), qkv_d=64, n_ctx=4, slots=2)
+    with pytest.raises(ValueError, match="1..80 rows"):
+        engine.debug_gemv_desc(np.zeros((81, 64), np.float16), w, mode=engine.GV_F32, out=np.zeros(81 * 128, np.float32), ldo=128)
+
+
 def test_no_cpu_fallback():
     if engine.device_count() > 0:
         pytest.skip("a GPU is present")
