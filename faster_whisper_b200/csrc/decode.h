@@ -49,7 +49,6 @@ struct SelfAttnArgs {
   __half* out;            // [R][d]
   int d, n_ctx, slots;
   long long anc_buf_stride;
-  int step_base;          // unused (kept for ABI stability of the struct)
 };
 void dec_self_attn(const SelfAttnArgs& a, int R, int H, cudaStream_t s);
 

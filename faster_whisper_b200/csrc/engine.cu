@@ -68,6 +68,29 @@ static T* model_alloc(Model* m, size_t n) {
   return p;
 }
 
+// Scratch device buffers of one call, freed when the call returns or throws.
+struct ScratchBufs {
+  std::vector<void*> ptrs;
+  ~ScratchBufs() {
+    for (void* p : ptrs) cudaFree(p);
+  }
+  template <typename T>
+  T* alloc(size_t n) {
+    T* p = dalloc<T>(n);
+    ptrs.push_back(p);
+    return p;
+  }
+  // n_dev elements (at least n_host), zeroed, then the first n_host copied from `host` (nothing when it is NULL)
+  template <typename T>
+  T* put(const void* host, size_t n_host, size_t n_dev = 0) {
+    n_dev = std::max(n_dev, n_host);
+    T* p = alloc<T>(n_dev);
+    B2W_CUDA(cudaMemset(p, 0, std::max<size_t>(n_dev, 1) * sizeof(T)));
+    if (host && n_host) B2W_CUDA(cudaMemcpy(p, host, n_host * sizeof(T), cudaMemcpyHostToDevice));
+    return p;
+  }
+};
+
 Model::~Model() {
   cudaSetDevice(device);
   if (stream) cudaStreamSynchronize(stream);
@@ -303,6 +326,14 @@ static __half* upload_conv(Uploader& up, const TensorTable& tt, const std::strin
   return p;
 }
 
+// every head of the last half of the decoder (OpenAI Whisper's default)
+static std::vector<int2> default_alignment_heads(const b2w_config& c) {
+  std::vector<int2> v;
+  for (int l = c.n_text_layer / 2; l < c.n_text_layer; ++l)
+    for (int hd = 0; hd < c.n_text_head; ++hd) v.push_back(make_int2(l, hd));
+  return v;
+}
+
 static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) {
   m->cfg = cfg;
   const int d = cfg.n_audio_state, dt = cfg.n_text_state;
@@ -369,7 +400,6 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     const std::string p = "decoder.blocks." + std::to_string(i);
     DecLayerW& D = m->dec[i];
     // LayerNorm affines are folded into the consuming projections (fold_ln); the kernels normalise only
-    D.ln1_g = D.ln1_b = D.ln2_g = D.ln2_b = D.ln3_g = D.ln3_b = nullptr;
     {
       const std::vector<float> g1 = host_f32(tt.get(p + ".attn_ln.weight")), b1 = host_f32(tt.get(p + ".attn_ln.bias"));
       expect_shape(tt.get(p + ".attn_ln.weight"), {dt});
@@ -435,7 +465,6 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     m->logit_b = up.alloc<float>((size_t)m->vpad);
     up.vec_to_f16(E, m->logit_w);
     up.vec_to_f32(lb, m->logit_b);
-    m->dec_ln_g = m->dec_ln_b = nullptr;
   }
   m->dec_weight_bytes = wbytes;
   m->mel.reset(new MelPlan(cfg.n_mels));
@@ -546,8 +575,7 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     m->d_bar = model_alloc<unsigned>(m, kBsBarWords);
     B2W_CUDA(cudaMemset(m->d_bar, 0, kBsBarWords * sizeof(unsigned)));
   }
-  for (int l = L / 2; l < L; ++l)  // default alignment heads: every head of the last half of the decoder (OpenAI Whisper's default)
-    for (int hh = 0; hh < cfg.n_text_head; ++hh) m->align_heads.push_back(make_int2(l, hh));
+  m->align_heads = default_alignment_heads(cfg);
   B2W_CUDA(cudaStreamSynchronize(m->stream));
 }
 
@@ -686,27 +714,23 @@ static void encoder_forward(Model* m, int b, __half* dst) {
 
 constexpr int kEncSub = 16;  // chunks per encoder pass (workspace ~70 MB per chunk at large-v3)
 
-static Encoded* encode_features(Model* m, const float* feats_host, const float* feats_dev, int B) {
+// Encoder output of B chunks, in sub-batches of kEncSub: fill(b0, b) puts the features of chunks b0 .. b0+b into m->e_feats.
+template <typename F>
+static std::unique_ptr<Encoded> encode(Model* m, int B, F&& fill) {
   std::unique_ptr<Encoded> e(new Encoded);
   e->owner = m;
   e->B = B;
   const size_t d = m->cfg.n_audio_state;
   e->enc_bytes = (size_t)B * 1500 * d * sizeof(__half);
   e->enc_out = reinterpret_cast<__half*>(m->pool_get(e->enc_bytes));
-  const size_t per = (size_t)m->cfg.n_mels * 3000;
   for (int b0 = 0; b0 < B; b0 += kEncSub) {
     const int b = std::min(kEncSub, B - b0);
     ensure_encoder_ws(m, std::min(kEncSub, B));
-    if (feats_host) {
-      ScopedStage st(m, B2W_T_H2D);
-      B2W_CUDA(cudaMemcpyAsync(m->e_feats, feats_host + b0 * per, b * per * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    } else if (feats_dev != m->e_feats) {
-      B2W_CUDA(cudaMemcpyAsync(m->e_feats, feats_dev + b0 * per, b * per * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-    }
+    fill(b0, b);
     ScopedStage st(m, B2W_T_ENCODER);
     encoder_forward(m, b, e->enc_out + (size_t)b0 * 1500 * d);
   }
-  return e.release();
+  return e;
 }
 
 // ---- log-mel --------------------------------------------------------------------------------------------------------------
@@ -833,6 +857,13 @@ static void ensure_cross_kv(Model* m, Encoded* e) {
   }
 }
 
+// Decoder and search workspaces for groups of `chunks` chunks x K rows, and the cross-attention K/V of `e` (none for fake logits).
+static void prepare_decode(Model* m, Encoded* e, int chunks, int K) {
+  ensure_decoder_ws(m, chunks, K);
+  ensure_search_ws(m, chunks, K);
+  if (e) ensure_cross_kv(m, e);
+}
+
 constexpr int kTcMinRows = 17;  // rows above which the decode GEMMs go through the wgmma path (activations reused from smem)
 
 // whether a decode GEMM goes through the tensor-core GEMM (else the skinny mma.sync kernel)
@@ -924,13 +955,23 @@ static void ensure_xpart(Model* m, size_t floats) {
   m->d_xpart_floats = floats;
 }
 
+// Whisper.align: the cross-attention probabilities of the alignment heads for the rows of one forced-decoding pass of one chunk,
+// row r written to out[head][pos0 + r][0..nf) of an [n_heads][n_tok][nf] buffer.
+struct AlignCapture {
+  const int2* heads;
+  int n_heads;
+  float* out;
+  int n_tok, nf, pos0;
+};
+
 // The layered decoder step: one launch per GEMM / attention.  Needs ensure_xpart(m, xpart_floats(m, n_chunks, rows_per_chunk)).
-static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots) {
+// Every LayerNorm normalises only: the affines are folded into the projections that consume them (fold_ln).
+static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots, const AlignCapture* cap) {
   const b2w_config& c = m->cfg;
   const int dt = c.n_text_state, L = c.n_text_layer, H = c.n_text_head, R = n_chunks * rows_per_chunk;
   cudaStream_t s = m->stream;
   const SearchBuffers& sb = m->sb;
-  embed_ln(sb.tokens_in, sb.rows, m->tok_emb, m->dec_pos, m->dec[0].ln1_g, m->dec[0].ln1_b, m->d_x, m->d_xn, R, dt, c.n_vocab, s);
+  embed_ln(sb.tokens_in, sb.rows, m->tok_emb, m->dec_pos, nullptr, nullptr, m->d_x, m->d_xn, R, dt, c.n_vocab, s);
   const int qgroups = cross_attn_qgroups(rows_per_chunk);
   B2W_CHECK(m->d_xpart_floats >= xpart_floats(m, n_chunks, rows_per_chunk), "cross-attention partial buffer");
   B2W_CHECK((size_t)n_chunks * H * qgroups <= 16 * 20 * 64, "cross-attention group counters");
@@ -942,18 +983,16 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     a.x = m->d_xn; a.W = W.wqkv; a.bias = W.bqkv; a.R = R; a.N = 3 * dt; a.K = dt; a.mode = GV_QKV;
     a.rows = sb.rows; a.kcache = kc; a.vcache = vc; a.d = dt; a.n_ctx = c.n_text_ctx; a.slots = slots; a.out_h = m->d_q;
     gv(m, a);
-    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots, (long long)n_chunks * slots * c.n_text_ctx, 0};
+    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots, (long long)n_chunks * slots * c.n_text_ctx};
     dec_self_attn(sa, R, H, s);
     GvArgs o;
     o.x = m->d_ao; o.W = W.wo; o.bias = W.bo; o.R = R; o.N = dt; o.K = dt; o.mode = GV_RESID_LN;
-    o.xres = m->d_x; o.ln_g = W.ln2_g; o.ln_b = W.ln2_b; o.xn_out = m->d_xn; o.counter = m->d_counters;
+    o.xres = m->d_x; o.xn_out = m->d_xn; o.counter = m->d_counters;
     gv(m, o);
     GvArgs q;
     q.x = m->d_xn; q.W = W.wq_x; q.bias = W.bq_x; q.R = R; q.N = dt; q.K = dt; q.mode = GV_F16; q.out_h = m->d_q;
     gv(m, q);
-    if (m->align_out)
-      align_probs(m->d_q, m->d_bind, l, m->d_align_heads, (int)m->align_heads.size(), m->align_out, m->align_n_tok, m->align_nf,
-                  m->align_pos0, R, H, 1500, dt, s);
+    if (cap) align_probs(m->d_q, m->d_bind, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, cap->pos0, R, H, 1500, dt, s);
     if (dstep_cross_attn_supported(1500, rows_per_chunk)) {
       DStepArgs xa{};
       xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
@@ -970,17 +1009,14 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     }
     GvArgs ox;
     ox.x = m->d_ao; ox.W = W.wo_x; ox.bias = W.bo_x; ox.R = R; ox.N = dt; ox.K = dt; ox.mode = GV_RESID_LN;
-    ox.xres = m->d_x; ox.ln_g = W.ln3_g; ox.ln_b = W.ln3_b; ox.xn_out = m->d_xn; ox.counter = m->d_counters;
+    ox.xres = m->d_x; ox.xn_out = m->d_xn; ox.counter = m->d_counters;
     gv(m, ox);
     GvArgs f1;
     f1.x = m->d_xn; f1.W = W.w1; f1.bias = W.b1; f1.R = R; f1.N = 4 * dt; f1.K = dt; f1.mode = GV_GELU_F16; f1.out_h = m->d_h;
     gv(m, f1);
     GvArgs f2;
     f2.x = m->d_h; f2.W = W.w2; f2.bias = W.b2; f2.R = R; f2.N = dt; f2.K = 4 * dt; f2.mode = GV_RESID_LN;
-    f2.xres = m->d_x;
-    f2.ln_g = (l + 1 < L) ? m->dec[l + 1].ln1_g : m->dec_ln_g;
-    f2.ln_b = (l + 1 < L) ? m->dec[l + 1].ln1_b : m->dec_ln_b;
-    f2.xn_out = m->d_xn; f2.counter = m->d_counters;
+    f2.xres = m->d_x; f2.xn_out = m->d_xn; f2.counter = m->d_counters;
     gv(m, f2);
   }
 }
@@ -992,22 +1028,33 @@ static void logits_gemm(Model* m, int R) {
   gv(m, a);
 }
 
-// Forced decoding of tokens[chunk][i0..i1) for chunks [chunk0, chunk0+n): rows = n*(i1-i0) <= 80, slot 0.
-static void prefill_pass(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int i0, int i1, int slots) {
-  const int rpc = i1 - i0, R = n * rpc;
-  std::vector<RowInfo> rows(R);
-  std::vector<int> toks(R);
-  for (int b = 0; b < n; ++b)
-    for (int i = i0; i < i1; ++i) {
-      rows[b * rpc + (i - i0)] = RowInfo{b, 0, i, 0};
-      toks[b * rpc + (i - i0)] = tokens[(size_t)(chunk0 + b) * stride + i];
-    }
-  B2W_CUDA(cudaMemcpyAsync(m->sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, m->stream));
-  B2W_CUDA(cudaMemcpyAsync(m->sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  B2W_CUDA(cudaStreamSynchronize(m->stream));  // host vectors go out of scope
-  bind_encoded(m, e, chunk0);
-  ensure_xpart(m, xpart_floats(m, n, rpc));
-  decoder_layers(m, n, rpc, slots);
+// Forced decoding of tokens[b * stride + i], i < n_tok, for chunks chunk0 .. chunk0+n of `e`, in passes of max(1, 80 / n)
+// positions; every row writes self-KV slot 0 of `slots`.  The slot ancestry must be zero: clear_anc zeroes it, unless the caller
+// already has.  When `cap` is set, every pass captures the alignment heads' cross-attention (cap->pos0 is set per pass).
+// After each pass's decoder layers, on_pass(i0, i1) may run logits_gemm: row b * (i1 - i0) + (i - i0) holds position i of chunk b.
+template <typename F>
+static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int n_tok, int slots,
+                          bool clear_anc, AlignCapture* cap, F&& on_pass) {
+  if (clear_anc) B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * slots * m->cfg.n_text_ctx, m->stream));
+  const int per_pass = std::max(1, kMaxRows / n);
+  for (int i0 = 0; i0 < n_tok; i0 += per_pass) {
+    const int i1 = std::min(n_tok, i0 + per_pass), rpc = i1 - i0, R = n * rpc;
+    std::vector<RowInfo> rows(R);
+    std::vector<int> toks(R);
+    for (int b = 0; b < n; ++b)
+      for (int i = i0; i < i1; ++i) {
+        rows[b * rpc + (i - i0)] = RowInfo{b, 0, i, 0};
+        toks[b * rpc + (i - i0)] = tokens[(size_t)b * stride + i];
+      }
+    B2W_CUDA(cudaMemcpyAsync(m->sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, m->stream));
+    B2W_CUDA(cudaMemcpyAsync(m->sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    B2W_CUDA(cudaStreamSynchronize(m->stream));  // host vectors go out of scope
+    bind_encoded(m, e, chunk0);
+    ensure_xpart(m, xpart_floats(m, n, rpc));
+    if (cap) cap->pos0 = i0;
+    decoder_layers(m, n, rpc, slots, cap);
+    on_pass(i0, i1);
+  }
 }
 
 // ---- generate: one group of n chunks x K rows --------------------------------------------------------------------------------
@@ -1058,19 +1105,16 @@ static SearchParams search_params(const Model* m, const int32_t* prompts, int n,
   return sp;
 }
 
-// Prompt[:-1] of every chunk in passes of <= 80 rows; the no-speech probability comes from the pass that holds the SOT row.
+// Prompt[:-1] of every chunk of the group; the no-speech probability comes from the pass that holds the SOT row.  The search
+// reset has cleared the slot ancestry.
 static void prefill(Model* m, const Encoded* e, int chunk0, int n, const int32_t* prompts, int P, int K, int sot_index, bool no_speech) {
   ScopedStage st(m, B2W_T_PREFILL);
   const b2w_config& c = m->cfg;
-  const int per_pass = std::max(1, kMaxRows / n);
-  for (int i0 = 0; i0 < P - 1; i0 += per_pass) {
-    const int i1 = std::min(P - 1, i0 + per_pass);
-    prefill_pass(m, e, chunk0, n, prompts, P, i0, i1, K);
-    if (no_speech && sot_index >= i0 && sot_index < i1) {
-      logits_gemm(m, n * (i1 - i0));
-      no_speech_from_logits(m->d_logits, m->vpad, n * (i1 - i0), i1 - i0, sot_index - i0, c.n_vocab, c.no_speech, m->sb.no_speech, m->stream);
-    }
-  }
+  forced_decode(m, e, chunk0, n, prompts + (size_t)chunk0 * P, P, P - 1, K, false, nullptr, [&](int i0, int i1) {
+    if (!no_speech || sot_index < i0 || sot_index >= i1) return;
+    logits_gemm(m, n * (i1 - i0));
+    no_speech_from_logits(m->d_logits, m->vpad, n * (i1 - i0), i1 - i0, sot_index - i0, c.n_vocab, c.no_speech, m->sb.no_speech, m->stream);
+  });
 }
 
 struct Step {  // one decode step of a chunk group: its path and the argument block of a persistent kernel
@@ -1158,7 +1202,7 @@ static void launch_decoder(Model* m, const Step& st) {
     case StepPath::Dstep: dstep_launch(st.ds, m->dstep_grid, m->stream); break;
     case StepPath::Bstep: bstep_launch(st.bs, m->num_sms, m->stream); break;
     case StepPath::Layers:
-      decoder_layers(m, st.n, st.K, st.K);
+      decoder_layers(m, st.n, st.K, st.K, nullptr);
       logits_gemm(m, R);
       break;
   }
@@ -1346,6 +1390,25 @@ struct b2w_encoded {
   Encoded* e;
 };
 
+// Runs f(m) with calls on the model serialised, its device current and the kernels f launches added to its counter.
+template <typename F>
+static void with_model(Model* m, F&& f) {
+  std::lock_guard<std::mutex> lk(m->mu);
+  DeviceGuard g(m->device);
+  const int64_t before = g_launches;
+  f(m);
+  m->launches += g_launches - before;
+}
+
+// An entry point that works on a model.  f validates its arguments before any device work.
+template <typename F>
+static int guarded(b2w_model* h, F&& f) {
+  return guarded([&] {
+    B2W_CHECK(h, "null model");
+    with_model(&h->m, f);
+  });
+}
+
 // ---- helpers of the test hooks ----------------------------------------------------------------------------------------
 static_assert(B2W_EPI_F16 == EPI_F16 && B2W_EPI_GELU_F16 == EPI_GELU_F16 && B2W_EPI_RESID_F32 == EPI_RESID_F32 &&
                   B2W_EPI_GELU_POS_F32 == EPI_GELU_POS_F32 && B2W_EPI_F16_XKV == EPI_F16_XKV && B2W_EPI_F32 == EPI_F32 &&
@@ -1353,23 +1416,6 @@ static_assert(B2W_EPI_F16 == EPI_F16 && B2W_EPI_GELU_F16 == EPI_GELU_F16 && B2W_
 static_assert(B2W_GV_QKV == GV_QKV && B2W_GV_F16 == GV_F16 && B2W_GV_GELU_F16 == GV_GELU_F16 && B2W_GV_RESID_LN == GV_RESID_LN &&
                   B2W_GV_F32 == GV_F32, "public decode GEMM modes");
 
-// Device copies of a test hook's host buffers, freed when the hook returns or throws.
-struct HookBufs {
-  std::vector<void*> ptrs;
-  ~HookBufs() {
-    for (void* p : ptrs) cudaFree(p);
-  }
-  // n_dev elements (at least n_host), zeroed, then the first n_host copied from `host` (nothing when it is NULL)
-  template <typename T>
-  T* put(const void* host, size_t n_host, size_t n_dev = 0) {
-    n_dev = std::max(n_dev, n_host);
-    T* p = dalloc<T>(n_dev);
-    ptrs.push_back(p);
-    B2W_CUDA(cudaMemset(p, 0, std::max<size_t>(n_dev, 1) * sizeof(T)));
-    if (host && n_host) B2W_CUDA(cudaMemcpy(p, host, n_host * sizeof(T), cudaMemcpyHostToDevice));
-    return p;
-  }
-};
 static void hook_get(void* host, const void* dev, size_t bytes) {
   if (host) B2W_CUDA(cudaMemcpy(host, dev, bytes, cudaMemcpyDeviceToHost));
 }
@@ -1439,6 +1485,7 @@ int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n
 
 void b2w_model_destroy(b2w_model* m) { delete m; }
 
+// reads only what b2w_model_create fixed, so it neither waits for the model nor touches the device
 int b2w_model_info(const b2w_model* m, b2w_config* cfg_out, int32_t* device_out) {
   return guarded([&] {
     B2W_CHECK(m, "null model");
@@ -1448,11 +1495,7 @@ int b2w_model_info(const b2w_model* m, b2w_config* cfg_out, int32_t* device_out)
 }
 
 int b2w_model_sync(b2w_model* h) {
-  return guarded([&] {
-    B2W_CHECK(h, "null model");
-    DeviceGuard g(h->m.device);
-    B2W_CUDA(cudaStreamSynchronize(h->m.stream));
-  });
+  return guarded(h, [&](Model* m) { B2W_CUDA(cudaStreamSynchronize(m->stream)); });
 }
 
 int b2w_logmel_frames(int64_t n_samples, int32_t padding) {
@@ -1476,62 +1519,43 @@ int b2w_logmel(int32_t device, int32_t n_mels, const float* pcm, int64_t n_sampl
     if (n_frames == 0) return;
     cudaStream_t s = nullptr;
     B2W_CUDA(cudaStreamCreate(&s));
-    float* d_pcm = dalloc<float>(n_samples);
-    float* d_out = dalloc<float>((size_t)n_frames * n_mels);
-    MelChunkDesc* d_desc = dalloc<MelChunkDesc>(1);
-    int* d_max = dalloc<int>(1);
-    try {
-      if (n_samples) B2W_CUDA(cudaMemcpyAsync(d_pcm, pcm, n_samples * 4, cudaMemcpyHostToDevice, s));
-      MelChunkDesc desc{d_pcm, n_samples, n_frames, n_frames};
-      B2W_CUDA(cudaMemcpyAsync(d_desc, &desc, sizeof desc, cudaMemcpyHostToDevice, s));
-      plan->run(d_desc, 1, n_frames, padding, d_out, 0, n_frames, d_max, false, s);
-      B2W_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n_frames * n_mels * 4, cudaMemcpyDeviceToHost, s));
-      B2W_CUDA(cudaStreamSynchronize(s));
-    } catch (...) {
-      cudaFree(d_pcm); cudaFree(d_out); cudaFree(d_desc); cudaFree(d_max); cudaStreamDestroy(s);
-      throw;
-    }
-    cudaFree(d_pcm); cudaFree(d_out); cudaFree(d_desc); cudaFree(d_max); cudaStreamDestroy(s);
+    std::unique_ptr<CUstream_st, decltype(&cudaStreamDestroy)> own_s(s, cudaStreamDestroy);  // destroyed after the buffers
+    ScratchBufs sb;
+    float* d_pcm = sb.alloc<float>(n_samples);
+    float* d_out = sb.alloc<float>((size_t)n_frames * n_mels);
+    MelChunkDesc* d_desc = sb.alloc<MelChunkDesc>(1);
+    int* d_max = sb.alloc<int>(1);
+    if (n_samples) B2W_CUDA(cudaMemcpyAsync(d_pcm, pcm, n_samples * 4, cudaMemcpyHostToDevice, s));
+    MelChunkDesc desc{d_pcm, n_samples, n_frames, n_frames};
+    B2W_CUDA(cudaMemcpyAsync(d_desc, &desc, sizeof desc, cudaMemcpyHostToDevice, s));
+    plan->run(d_desc, 1, n_frames, padding, d_out, 0, n_frames, d_max, false, s);
+    B2W_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n_frames * n_mels * 4, cudaMemcpyDeviceToHost, s));
+    B2W_CUDA(cudaStreamSynchronize(s));
   });
 }
 
 int b2w_encode(b2w_model* h, const float* features, int32_t batch, b2w_encoded** out) {
-  return guarded([&] {
-    B2W_CHECK(h && features && out && batch > 0, "bad encode arguments");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
-    const int64_t before = g_launches;
-    std::unique_ptr<b2w_encoded> r(new b2w_encoded);
-    r->e = encode_features(m, features, nullptr, batch);
-    m->launches += g_launches - before;
-    *out = r.release();
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(features && out && batch > 0, "bad encode arguments");
+    const size_t per = (size_t)m->cfg.n_mels * 3000;
+    std::unique_ptr<Encoded> e = encode(m, batch, [&](int b0, int b) {
+      ScopedStage st(m, B2W_T_H2D);
+      B2W_CUDA(cudaMemcpyAsync(m->e_feats, features + b0 * per, b * per * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    });
+    *out = new b2w_encoded{e.release()};
   });
 }
 
 int b2w_encode_audio(b2w_model* h, const float* const* pcm, const int64_t* n_samples, int32_t batch, float* features_out,
                      b2w_encoded** out) {
-  return guarded([&] {
-    B2W_CHECK(h && pcm && n_samples && out && batch > 0, "bad encode_audio arguments");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
-    const int64_t before = g_launches;
-    const int n_mels = m->cfg.n_mels;
-    const size_t per = (size_t)n_mels * 3000, d = m->cfg.n_audio_state;
-    std::unique_ptr<Encoded> e(new Encoded);
-    e->owner = m;
-    e->B = batch;
-    e->enc_bytes = (size_t)batch * 1500 * d * sizeof(__half);
-    e->enc_out = reinterpret_cast<__half*>(m->pool_get(e->enc_bytes));
-    for (int b0 = 0; b0 < batch; b0 += kEncSub) {
-      const int b = std::min(kEncSub, batch - b0);
-      ensure_encoder_ws(m, std::min(kEncSub, (int)batch));
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(pcm && n_samples && out && batch > 0, "bad encode_audio arguments");
+    for (int i = 0; i < batch; ++i)
+      B2W_CHECK(n_samples[i] >= 0 && n_samples[i] <= 480000, "a chunk holds at most 30 s of 16 kHz audio");
+    const size_t per = (size_t)m->cfg.n_mels * 3000;
+    std::unique_ptr<Encoded> e = encode(m, batch, [&](int b0, int b) {
       size_t total = 0;
-      for (int i = 0; i < b; ++i) {
-        B2W_CHECK(n_samples[b0 + i] >= 0 && n_samples[b0 + i] <= 480000, "a chunk holds at most 30 s of 16 kHz audio");
-        total += (n_samples[b0 + i] + 3) & ~size_t(3);
-      }
+      for (int i = 0; i < b; ++i) total += (n_samples[b0 + i] + 3) & ~size_t(3);
       if (total > m->e_pcm_cap) {
         B2W_CUDA(cudaStreamSynchronize(m->stream));
         if (m->e_pcm) cudaFree(m->e_pcm);
@@ -1563,13 +1587,8 @@ int b2w_encode_audio(b2w_model* h, const float* const* pcm, const int64_t* n_sam
         B2W_CUDA(cudaMemcpyAsync(features_out + (size_t)b0 * per, m->e_feats, (size_t)b * per * 4, cudaMemcpyDeviceToHost, m->stream));
       }
       B2W_CUDA(cudaStreamSynchronize(m->stream));  // desc vector lifetime
-      ScopedStage st(m, B2W_T_ENCODER);
-      encoder_forward(m, b, e->enc_out + (size_t)b0 * 1500 * d);
-    }
-    m->launches += g_launches - before;
-    std::unique_ptr<b2w_encoded> r(new b2w_encoded);
-    r->e = e.release();
-    *out = r.release();
+    });
+    *out = new b2w_encoded{e.release()};
   });
 }
 
@@ -1583,37 +1602,33 @@ int b2w_encoded_shape(const b2w_encoded* e, int64_t shape_out[3]) {
 }
 
 int b2w_encoded_to_host(b2w_model* h, const b2w_encoded* e, float* out) {
-  return guarded([&] {
-    B2W_CHECK(h && e && e->e && out, "bad arguments");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(e && e->e && out, "bad arguments");
     const size_t n = (size_t)e->e->B * 1500 * m->cfg.n_audio_state;
-    float* tmp = dalloc<float>(n);
+    ScratchBufs sb;
+    float* tmp = sb.alloc<float>(n);
     convert_f16_f32(e->e->enc_out, tmp, n, m->stream);
     B2W_CUDA(cudaMemcpyAsync(out, tmp, n * 4, cudaMemcpyDeviceToHost, m->stream));
     B2W_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(tmp);
   });
 }
 
 void b2w_encoded_free(b2w_encoded* e) {
   if (!e) return;
-  if (e->e) {
-    Model* m = e->e->owner;
-    std::lock_guard<std::mutex> lk(m->mu);
-    cudaSetDevice(m->device);
-    cudaStreamSynchronize(m->stream);
-    delete e->e;
-  }
+  if (e->e)  // the owner's stream may still read the output; ~Encoded returns its buffers to the owner's pool
+    guarded([&] {
+      with_model(e->e->owner, [&](Model* m) {
+        cudaStreamSynchronize(m->stream);
+        delete e->e;
+      });
+    });
   delete e;
 }
 
 int b2w_generate(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t prompt_len, int32_t batch,
                  const b2w_gen_opts* opts, int32_t* out_ids, int32_t* out_lens, float* out_scores, float* out_no_speech) {
-  return guarded([&] {
-    B2W_CHECK(h && prompts && opts && out_ids && out_lens && out_scores && out_no_speech, "null argument");
-    Model* m = &h->m;
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(prompts && opts && out_ids && out_lens && out_scores && out_no_speech, "null argument");
     const b2w_gen_opts& o = *opts;
     B2W_CHECK(batch > 0 && prompt_len > 0, "empty batch or prompt");
     B2W_CHECK(o.debug_fake_logits || (enc && enc->e && enc->e->B == batch), "one prompt per encoder output row is required");
@@ -1623,9 +1638,6 @@ int b2w_generate(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t
     B2W_CHECK(o.max_length >= 1 && o.max_length <= m->cfg.n_text_ctx, "max_length must be in 1..n_text_ctx");
     B2W_CHECK(o.sampling_topk == 0 || o.sampling_topk == 1, "sampling_topk must be 0 (full vocabulary) or 1 (argmax)");
     B2W_CHECK(o.patience > 0 && o.repetition_penalty > 0, "patience and repetition_penalty must be positive");
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
-    const int64_t before = g_launches;
     const int K = o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
     const int group = std::max(1, kMaxRows / K);
     // suppress mask
@@ -1639,46 +1651,34 @@ int b2w_generate(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t
       B2W_CUDA(cudaMemcpyAsync(m->d_suppress, mask.data(), m->vpad, cudaMemcpyHostToDevice, m->stream));
       B2W_CUDA(cudaStreamSynchronize(m->stream));
     }
-    ensure_decoder_ws(m, std::min(group, (int)batch), K);
-    ensure_search_ws(m, std::min(group, (int)batch), K);
-    m->sb.suppress = m->d_suppress;
-    std::unique_ptr<Encoded> dummy;
     Encoded* e = enc ? enc->e : nullptr;
-    if (!o.debug_fake_logits) ensure_cross_kv(m, e);
+    prepare_decode(m, o.debug_fake_logits ? nullptr : e, std::min(group, (int)batch), K);
     for (int c0 = 0; c0 < batch; c0 += group) {
       const int n = std::min(group, batch - c0);
       generate_group(m, e, c0, n, prompts, prompt_len, o, out_ids, out_lens, out_scores, out_no_speech);
     }
-    m->launches += g_launches - before;
   });
 }
 
 int b2w_detect_language(b2w_model* h, b2w_encoded* enc, float* probs) {
-  return guarded([&] {
-    B2W_CHECK(h && enc && enc->e && probs, "null argument");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
-    const int64_t before = g_launches;
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && probs, "null argument");
     Encoded* e = enc->e;
     const int nl = m->cfg.num_languages;
-    ensure_cross_kv(m, e);
     const int group = kMaxRows;
-    ensure_decoder_ws(m, std::min(group, e->B), 1);
-    ensure_search_ws(m, std::min(group, e->B), 1);
-    float* d_probs = dalloc<float>((size_t)e->B * nl);
-    std::vector<int32_t> toks(e->B, m->cfg.sot);
+    prepare_decode(m, e, std::min(group, e->B), 1);
+    ScratchBufs sb;
+    float* d_probs = sb.alloc<float>((size_t)e->B * nl);
+    const std::vector<int32_t> sot(group, m->cfg.sot);
     for (int c0 = 0; c0 < e->B; c0 += group) {
       const int n = std::min(group, e->B - c0);
-      B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * m->cfg.n_text_ctx, m->stream));
-      prefill_pass(m, e, c0, n, toks.data(), 1, 0, 1, 1);
-      logits_gemm(m, n);
-      lang_probs_from_logits(m->d_logits, m->vpad, n, m->cfg.lang_begin, nl, d_probs + (size_t)c0 * nl, m->stream);
+      forced_decode(m, e, c0, n, sot.data(), 1, 1, 1, true, nullptr, [&](int, int) {
+        logits_gemm(m, n);
+        lang_probs_from_logits(m->d_logits, m->vpad, n, m->cfg.lang_begin, nl, d_probs + (size_t)c0 * nl, m->stream);
+      });
     }
     B2W_CUDA(cudaMemcpyAsync(probs, d_probs, (size_t)e->B * nl * 4, cudaMemcpyDeviceToHost, m->stream));
     B2W_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(d_probs);
-    m->launches += g_launches - before;
   });
 }
 
@@ -1739,22 +1739,16 @@ static void dtw_path(const std::vector<double>& c, int N, int M, std::vector<int
 }
 
 int b2w_model_set_alignment_heads(b2w_model* h, const int32_t* layer_head_pairs, int32_t n_pairs) {
-  return guarded([&] {
-    B2W_CHECK(h && (n_pairs == 0 || layer_head_pairs) && n_pairs >= 0 && n_pairs <= 32 * 32, "bad arguments");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK((n_pairs == 0 || layer_head_pairs) && n_pairs >= 0 && n_pairs <= 32 * 32, "bad arguments");
     std::vector<int2> v;
     for (int i = 0; i < n_pairs; ++i) {
       const int l = layer_head_pairs[2 * i], hd = layer_head_pairs[2 * i + 1];
       if (l < 0 || l >= m->cfg.n_text_layer || hd < 0 || hd >= m->cfg.n_text_head) throw Error("alignment head out of range", true);
       v.push_back(make_int2(l, hd));
     }
-    if (v.empty())
-      for (int l = m->cfg.n_text_layer / 2; l < m->cfg.n_text_layer; ++l)
-        for (int hd = 0; hd < m->cfg.n_text_head; ++hd) v.push_back(make_int2(l, hd));
-    m->align_heads = v;
+    m->align_heads = v.empty() ? default_alignment_heads(m->cfg) : v;
     if (m->d_align_heads) {
-      DeviceGuard g(m->device);
       cudaFree(m->d_align_heads);
       m->d_align_heads = nullptr;
     }
@@ -1764,9 +1758,8 @@ int b2w_model_set_alignment_heads(b2w_model* h, const int32_t* layer_head_pairs,
 int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t* start_sequence, int32_t n_start,
               const int32_t* text_tokens, int32_t n_text, int32_t num_frames, int32_t median_filter_width, int32_t* alignments_out,
               int32_t capacity_pairs, int32_t* n_pairs_out, float* text_token_probs_out) {
-  return guarded([&] {
-    B2W_CHECK(h && enc && enc->e && start_sequence && n_pairs_out && n_start >= 1 && n_text >= 0, "bad arguments");
-    Model* m = &h->m;
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && start_sequence && n_pairs_out && n_start >= 1 && n_text >= 0, "bad arguments");
     const b2w_config& c = m->cfg;
     Encoded* e = enc->e;
     if (batch_index < 0 || batch_index >= e->B) throw Error("align: batch index out of range", true);
@@ -1785,12 +1778,8 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
     for (int t : seq)
       if (t < 0 || t >= c.n_vocab) throw Error("align: token id out of range", true);
     const int nf = std::max(1, std::min(1500, (int)num_frames / 2));
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
     cudaStream_t s = m->stream;
-    ensure_cross_kv(m, e);
-    ensure_decoder_ws(m, 1, 1);
-    ensure_search_ws(m, 1, 1);
+    prepare_decode(m, e, 1, 1);
     const int n_heads = (int)m->align_heads.size();
     B2W_CHECK(n_heads > 0, "no alignment heads");
     if (!m->d_align_heads) {
@@ -1805,25 +1794,11 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
     for (int t = 0; t < n_text; ++t) targets[n_head_rows - 1 + t] = text_tokens[t];  // position p predicts token p + 1
     B2W_CUDA(cudaMemcpyAsync(d_targets, targets.data(), (size_t)n_tok * sizeof(int), cudaMemcpyHostToDevice, s));
     B2W_CUDA(cudaMemsetAsync(d_tp, 0, (size_t)n_tok * sizeof(float), s));
-    B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * c.n_text_ctx, s));
-    std::vector<int32_t> padded((size_t)(batch_index + 1) * n_tok, 0);  // prefill_pass indexes tokens by absolute chunk
-    std::copy(seq.begin(), seq.end(), padded.begin() + (size_t)batch_index * n_tok);
-    m->align_out = d_att;
-    m->align_n_tok = n_tok;
-    m->align_nf = nf;
-    try {
-      for (int i0 = 0; i0 < n_tok; i0 += kMaxRows) {
-        const int i1 = std::min(n_tok, i0 + kMaxRows);
-        m->align_pos0 = i0;
-        prefill_pass(m, e, batch_index, 1, padded.data(), n_tok, i0, i1, 1);
-        logits_gemm(m, i1 - i0);
-        row_target_probs(m->d_logits, m->vpad, i1 - i0, c.n_vocab, d_targets + i0, d_tp + i0, s);
-      }
-    } catch (...) {
-      m->align_out = nullptr;
-      throw;
-    }
-    m->align_out = nullptr;
+    AlignCapture cap{m->d_align_heads, n_heads, d_att, n_tok, nf, 0};
+    forced_decode(m, e, batch_index, 1, seq.data(), n_tok, n_tok, 1, true, &cap, [&](int i0, int i1) {
+      logits_gemm(m, i1 - i0);
+      row_target_probs(m->d_logits, m->vpad, i1 - i0, c.n_vocab, d_targets + i0, d_tp + i0, s);
+    });
     std::vector<float> att(n_att), tp(n_tok);
     B2W_CUDA(cudaMemcpyAsync(att.data(), d_att, n_att * sizeof(float), cudaMemcpyDeviceToHost, s));
     B2W_CUDA(cudaMemcpyAsync(tp.data(), d_tp, (size_t)n_tok * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -1868,11 +1843,7 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
 }
 
 int b2w_span_begin(b2w_model* h) {
-  return guarded([&] {
-    B2W_CHECK(h, "bad arguments");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
+  return guarded(h, [&](Model* m) {
     if (!m->span_a) {
       B2W_CUDA(cudaEventCreate(&m->span_a));
       B2W_CUDA(cudaEventCreate(&m->span_b));
@@ -1881,11 +1852,8 @@ int b2w_span_begin(b2w_model* h) {
   });
 }
 int b2w_span_end(b2w_model* h, double* ms_out) {
-  return guarded([&] {
-    B2W_CHECK(h && ms_out && h->m.span_a, "b2w_span_end without b2w_span_begin");
-    Model* m = &h->m;
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(ms_out && m->span_a, "b2w_span_end without b2w_span_begin");
     B2W_CUDA(cudaEventRecord(m->span_b, m->stream));
     B2W_CUDA(cudaEventSynchronize(m->span_b));
     float ms = 0.f;
@@ -1895,43 +1863,37 @@ int b2w_span_end(b2w_model* h, double* ms_out) {
 }
 
 int b2w_timing_enable(b2w_model* h, int32_t on) {
-  return guarded([&] {
-    B2W_CHECK(h, "null model");
-    drain_timers(&h->m);
-    h->m.timing = on != 0;
+  return guarded(h, [&](Model* m) {
+    drain_timers(m);
+    m->timing = on != 0;
   });
 }
 int b2w_timing_reset(b2w_model* h) {
-  return guarded([&] {
-    B2W_CHECK(h, "null model");
-    DeviceGuard g(h->m.device);
-    drain_timers(&h->m);
+  return guarded(h, [&](Model* m) {
+    drain_timers(m);
     for (int i = 0; i < B2W_T_COUNT; ++i) {
-      h->m.t_ms[i] = 0;
-      h->m.t_cnt[i] = 0;
+      m->t_ms[i] = 0;
+      m->t_cnt[i] = 0;
     }
-    h->m.launches = 0;
-    h->m.decode_steps = 0;
-    h->m.decode_alg_bytes = 0;
+    m->launches = 0;
+    m->decode_steps = 0;
+    m->decode_alg_bytes = 0;
   });
 }
 int b2w_timing_get(b2w_model* h, double ms_out[B2W_T_COUNT], int64_t counts_out[B2W_T_COUNT]) {
-  return guarded([&] {
-    B2W_CHECK(h, "null model");
-    DeviceGuard g(h->m.device);
-    drain_timers(&h->m);
+  return guarded(h, [&](Model* m) {
+    drain_timers(m);
     for (int i = 0; i < B2W_T_COUNT; ++i) {
-      ms_out[i] = h->m.t_ms[i];
-      if (counts_out) counts_out[i] = h->m.t_cnt[i];
+      ms_out[i] = m->t_ms[i];
+      if (counts_out) counts_out[i] = m->t_cnt[i];
     }
   });
 }
 int b2w_counters_get(b2w_model* h, int64_t* launches, int64_t* decode_steps, double* decode_alg_bytes) {
-  return guarded([&] {
-    B2W_CHECK(h, "null model");
-    if (launches) *launches = h->m.launches;
-    if (decode_steps) *decode_steps = h->m.decode_steps;
-    if (decode_alg_bytes) *decode_alg_bytes = h->m.decode_alg_bytes;
+  return guarded(h, [&](Model* m) {
+    if (launches) *launches = m->launches;
+    if (decode_steps) *decode_steps = m->decode_steps;
+    if (decode_alg_bytes) *decode_alg_bytes = m->decode_alg_bytes;
   });
 }
 
@@ -1972,7 +1934,7 @@ int b2w_debug_gemm(int32_t device, int32_t impl, b2w_gemm_desc* d) {
     }
     require_hopper(device);
     DeviceGuard g(device);
-    HookBufs hb;
+    ScratchBufs hb;
     const int64_t K = (int64_t)d->taps * d->k_per_tap;
     const size_t out_bytes = (size_t)d->out_elems * (f16_out ? 2 : 4);
     GemmArgs ga;
@@ -2031,8 +1993,9 @@ int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t 
     require_hopper(device);
     DeviceGuard g(device);
     const size_t n_in = (size_t)B * T * 3 * H * 64, n_out = (size_t)B * T * H * 64;
-    float *dq = dalloc<float>(n_in), *dof = dalloc<float>(n_out);
-    __half *hq = dalloc<__half>(n_in), *ho = dalloc<__half>(n_out);
+    ScratchBufs sb;
+    float *dq = sb.alloc<float>(n_in), *dof = sb.alloc<float>(n_out);
+    __half *hq = sb.alloc<__half>(n_in), *ho = sb.alloc<__half>(n_out);
     B2W_CUDA(cudaMemcpy(dq, qkv, n_in * 4, cudaMemcpyHostToDevice));
     convert_f32_f16(dq, hq, n_in, 0);
     if (impl == 0) {
@@ -2044,7 +2007,6 @@ int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t 
     convert_f16_f32(ho, dof, n_out, 0);
     B2W_CUDA(cudaDeviceSynchronize());
     B2W_CUDA(cudaMemcpy(out, dof, n_out * 4, cudaMemcpyDeviceToHost));
-    cudaFree(dq); cudaFree(dof); cudaFree(hq); cudaFree(ho);
   });
 }
 
@@ -2076,7 +2038,7 @@ int b2w_debug_gemv(int32_t device, int32_t impl, b2w_gemv_desc* d) {
     }
     require_hopper(device);
     DeviceGuard g(device);
-    HookBufs hb;
+    ScratchBufs hb;
     // zero-padded like the decoder's workspaces: the skinny kernel reads activations in 8-row groups up to kMaxRows rows and
     // weights in 16-row groups
     const int Np = ceil_div(N, 16) * 16;
@@ -2130,10 +2092,8 @@ int b2w_debug_gemv(int32_t device, int32_t impl, b2w_gemv_desc* d) {
 }
 
 int b2w_debug_fetch(b2w_model* h, int32_t which, float* out, int64_t n) {
-  return guarded([&] {
-    B2W_CHECK(h && out && n >= 0, "null argument");
-    Model* m = &h->m;
-    DeviceGuard g(m->device);
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(out && n >= 0, "null argument");
     B2W_CHECK(m->d_x, "no decoder workspace yet");
     B2W_CUDA(cudaStreamSynchronize(m->stream));
     const float* f32 = nullptr;
@@ -2161,43 +2121,34 @@ int b2w_debug_fetch(b2w_model* h, int32_t which, float* out, int64_t n) {
 }
 
 int b2w_debug_logits(b2w_model* h, b2w_encoded* enc, const int32_t* tokens, int32_t n_tok, int32_t batch, float* logits_out) {
-  return guarded([&] {
-    B2W_CHECK(h && enc && enc->e && tokens && logits_out && enc->e->B == batch, "bad arguments");
-    Model* m = &h->m;
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && tokens && logits_out && enc->e->B == batch, "bad arguments");
     B2W_CHECK(n_tok >= 1 && n_tok <= m->cfg.n_text_ctx, "token count");
     for (size_t i = 0; i < (size_t)batch * n_tok; ++i) B2W_CHECK(tokens[i] >= 0 && tokens[i] < m->cfg.n_vocab, "token id out of range");
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
     Encoded* e = enc->e;
-    ensure_cross_kv(m, e);
     const int V = m->cfg.n_vocab;
     const int group = std::min((int)batch, kMaxRows);
-    ensure_decoder_ws(m, group, 1);
-    ensure_search_ws(m, group, 1);
+    prepare_decode(m, e, group, 1);
     std::vector<float> tmp((size_t)kMaxRows * m->vpad);
     for (int c0 = 0; c0 < batch; c0 += group) {
       const int n = std::min(group, batch - c0);
-      B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * m->cfg.n_text_ctx, m->stream));
-      const int per_pass = std::max(1, kMaxRows / n);
-      for (int i0 = 0; i0 < n_tok; i0 += per_pass) {
-        const int i1 = std::min((int)n_tok, i0 + per_pass), rpc = i1 - i0;
-        prefill_pass(m, e, c0, n, tokens, n_tok, i0, i1, 1);
+      forced_decode(m, e, c0, n, tokens + (size_t)c0 * n_tok, n_tok, n_tok, 1, true, nullptr, [&](int i0, int i1) {
+        const int rpc = i1 - i0;
         logits_gemm(m, n * rpc);
         B2W_CUDA(cudaMemcpyAsync(tmp.data(), m->d_logits, (size_t)n * rpc * m->vpad * 4, cudaMemcpyDeviceToHost, m->stream));
         B2W_CUDA(cudaStreamSynchronize(m->stream));
         for (int b = 0; b < n; ++b)
           for (int i = i0; i < i1; ++i)
             memcpy(logits_out + ((size_t)(c0 + b) * n_tok + i) * V, tmp.data() + (size_t)(b * rpc + i - i0) * m->vpad, (size_t)V * 4);
-      }
+      });
     }
   });
 }
 
 int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t P, int32_t n, int32_t K, int32_t n_steps,
                           const int32_t* tokens, const int32_t* parents, float* logits_out) {
-  return guarded([&] {
-    B2W_CHECK(h && enc && enc->e && prompts && tokens && logits_out, "null argument");
-    Model* m = &h->m;
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && prompts && tokens && logits_out, "null argument");
     const b2w_config& c = m->cfg;
     B2W_CHECK(enc->e->B == n, "one prompt per encoder output row is required");
     B2W_CHECK(K >= 1 && K <= kMaxBeam, "rows per chunk must be in 1..16");
@@ -2208,17 +2159,12 @@ int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts
     for (size_t i = 0; i < (size_t)n_steps * R; ++i) B2W_CHECK(tokens[i] >= 0 && tokens[i] < V, "token id out of range");
     if (parents)
       for (size_t i = 0; i < (size_t)n_steps * R; ++i) B2W_CHECK(parents[i] >= 0 && parents[i] < K, "parent slot out of range");
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
     Step st = choose_step(m, n, K, false);
-    ensure_decoder_ws(m, n, K);
-    ensure_search_ws(m, n, K);
     Encoded* e = enc->e;
-    ensure_cross_kv(m, e);
+    prepare_decode(m, e, n, K);
     cudaStream_t s = m->stream;
     const SearchBuffers& sb = m->sb;
-    B2W_CUDA(cudaMemsetAsync(sb.anc, 0, (size_t)2 * R * n_ctx, s));
-    if (P > 1) prefill(m, e, 0, n, prompts, P, K, -1, false);
+    forced_decode(m, e, 0, n, prompts, P, P - 1, K, true, nullptr, [](int, int) {});  // the prompt's keys, as prefill writes them
     b2w_gen_opts o;
     b2w_gen_opts_default(&o);
     o.beam_size = K;

@@ -21,8 +21,7 @@ struct EncLayerW {
   __half *wqkv, *wo, *w1, *w2;
   float *bqkv, *bo, *b1, *b2;
 };
-struct DecLayerW {
-  float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *ln3_g, *ln3_b;
+struct DecLayerW {  // every LayerNorm affine is folded into the projection that consumes it (fold_ln)
   __half *wqkv, *wo, *wq_x, *wo_x, *w1, *w2;
   float *bqkv, *bo, *bq_x, *bo_x, *b1, *b2;
 };
@@ -78,7 +77,7 @@ struct Model {
   __half* tok_emb = nullptr;  // [vpad][d]
   __half* logit_w = nullptr;  // [vpad][d]  tied embedding scaled by the final LayerNorm's gamma
   float* logit_b = nullptr;   // [vpad]     E . beta_f
-  float *dec_pos = nullptr, *dec_ln_g = nullptr, *dec_ln_b = nullptr;
+  float* dec_pos = nullptr;
   std::vector<DecLayerW> dec;
   __half* wxkv = nullptr;  // [L*2d][d]
   float* bxkv = nullptr;   // [L*2d]
@@ -106,7 +105,6 @@ struct Model {
   std::map<std::tuple<const void*, const void*, int, int, const void*, const void*, const void*, int>, GemmPlan> dec_plans;
 
   // decoder workspace
-  int dw_rows = 0;
   size_t kv_elems = 0;        // per layer per K|V
   __half* kcache = nullptr;   // [L][kv_elems]
   __half* vcache = nullptr;
@@ -118,12 +116,10 @@ struct Model {
   int* d_counters = nullptr;  // [0]: GEMM ticket, [64..]: cross-attention groups
   uint8_t* d_suppress = nullptr;
   DecBindings* d_bind = nullptr;
-  // Whisper.align: (layer, head) pairs whose cross-attention is captured; while `align_out` is set, decoder_layers() writes
-  // the probabilities of the forced-decoding rows there
+  // Whisper.align: (layer, head) pairs whose cross-attention b2w_align captures; d_align_heads is their device copy, made on
+  // first use
   std::vector<int2> align_heads;
   int2* d_align_heads = nullptr;
-  float* align_out = nullptr;
-  int align_n_tok = 0, align_nf = 0, align_pos0 = 0;
   cudaEvent_t span_a = nullptr, span_b = nullptr;  // b2w_span_begin / b2w_span_end
   const __half* logit_tiles = nullptr;  // output embedding as the persistent step kernel's tile stream
   DLayer* d_layers = nullptr;   // device copy of the decoder layer pointer table (persistent step kernel)

@@ -87,21 +87,31 @@ def test_encode_rejects_bad_shapes(eng, micro):
 
 
 # ---- decoder math: teacher-forced logits ---------------------------------------------------------------------
-def test_teacher_forced_logits(micro, eng):
-    st = micro["tokens"]
-    feats = features_for(micro, 2, seed=7)
-    enc_o = micro["oracle"].encode(feats)
+def _check_teacher_forced(eng, m, n_chunks, n_text, seed):
+    st = m["tokens"]
+    feats = features_for(m, n_chunks, seed=seed)
+    enc_o = m["oracle"].encode(feats)
     rng = np.random.default_rng(5)
-    toks = np.concatenate([np.array([[st.sot, st.no_timestamps]] * 2), rng.integers(0, 50000, (2, 21))], axis=1).astype(np.int32)
+    toks = np.concatenate([np.array([[st.sot, st.no_timestamps]] * n_chunks), rng.integers(0, 50000, (n_chunks, n_text))], axis=1).astype(np.int32)
     import torch
 
-    o = micro["oracle"]
-    cache = [None] * micro["dims"].n_text_layer
-    want = o.decoder_forward(torch.from_numpy(toks).long(), 0, cache, o.cross_kv(enc_o), torch.arange(2)).numpy()
+    o = m["oracle"]
+    cache = [None] * m["dims"].n_text_layer
+    want = o.decoder_forward(torch.from_numpy(toks).long(), 0, cache, o.cross_kv(enc_o), torch.arange(n_chunks)).numpy()
     got = eng.debug_logits(eng.encode(feats), toks)
     assert got.shape == want.shape
     assert np.abs(got - want).max() < LOGIT_TOL, np.abs(got - want).max()
     assert (got.argmax(-1) == want.argmax(-1)).mean() > 0.95
+
+
+def test_teacher_forced_logits(micro, eng):
+    _check_teacher_forced(eng, micro, 2, 21, seed=7)
+
+
+def test_teacher_forced_logits_over_several_passes(micro, eng):
+    """3 chunks x 60 positions: forced decoding in passes of 80 // 3 = 26 positions (26, 26, 8), each pass's logits scattered back
+    to its positions."""
+    _check_teacher_forced(eng, micro, 3, 58, seed=8)
 
 
 # ---- search logic with the deterministic stand-in decoder (bit-level comparison of the decisions) -------------
@@ -233,21 +243,14 @@ def _jump_frames(pairs, n_rows):
     return [first[t] for t in range(n_rows)]
 
 
-@pytest.mark.parametrize("heads", [None, [(1, 0), (1, 1), (0, 1)]])
-def test_align_matches_oracle(micro_ml, eng_ml, heads):
-    st = micro_ml["tokens"]
-    o = micro_ml["oracle"]
-    feats = features_for(micro_ml, 2, seed=60)
-    rng = np.random.default_rng(3)
-    text = [rng.integers(100, 5000, 14).tolist(), rng.integers(100, 5000, 6).tolist()]
-    frames = [3000, 1800]
-    start = [st.sot, st.lang_begin, st.transcribe]
+def _check_align(eng, m, feats, start, text, frames, heads=None):
+    o = m["oracle"]
     want = o.align(o.encode(feats), start, text, frames, 7, alignment_heads=heads)
-    eng_ml.set_alignment_heads(heads)
+    eng.set_alignment_heads(heads)
     try:
-        got = eng_ml.align(eng_ml.encode(feats), start, text, frames, median_filter_width=7)
+        got = eng.align(eng.encode(feats), start, text, frames, median_filter_width=7)
     finally:
-        eng_ml.set_alignment_heads(None)
+        eng.set_alignment_heads(None)
     for w, g, toks, nf in zip(want, got, text, frames):
         assert np.allclose(g.text_token_probs, w.text_token_probs, rtol=0.1, atol=1e-6), (g.text_token_probs, w.text_token_probs)
         gi, wi = np.array(g.alignments), np.array(w.alignments)
@@ -258,8 +261,28 @@ def test_align_matches_oracle(micro_ml, eng_ml, heads):
         gj, wj = _jump_frames(g.alignments, len(toks) + 1), _jump_frames(w.alignments, len(toks) + 1)
         close = sum(abs(a - b) <= 2 for a, b in zip(gj, wj))
         assert close >= len(gj) - 1, (gj, wj)
+
+
+@pytest.mark.parametrize("heads", [None, [(1, 0), (1, 1), (0, 1)]])
+def test_align_matches_oracle(micro_ml, eng_ml, heads):
+    st = micro_ml["tokens"]
+    feats = features_for(micro_ml, 2, seed=60)
+    rng = np.random.default_rng(3)
+    text = [rng.integers(100, 5000, 14).tolist(), rng.integers(100, 5000, 6).tolist()]
+    frames = [3000, 1800]
+    start = [st.sot, st.lang_begin, st.transcribe]
+    _check_align(eng_ml, micro_ml, feats, start, text, frames, heads)
     with pytest.raises(ValueError):
         eng_ml.align(eng_ml.encode(feats), start, [text[0]], frames)
+
+
+def test_align_over_several_passes(micro_ml, eng_ml):
+    """Batch item 1 forces 3 start tokens + <|notimestamps|> + 120 text tokens + <|endoftext|> = 125 positions, in passes of 80
+    and 45: the second pass's cross-attention lands at rows 80..124 of the capture."""
+    st = micro_ml["tokens"]
+    rng = np.random.default_rng(8)
+    text = [rng.integers(100, 5000, 6).tolist(), rng.integers(100, 5000, 120).tolist()]
+    _check_align(eng_ml, micro_ml, features_for(micro_ml, 2, seed=62), [st.sot, st.lang_begin, st.transcribe], text, [3000, 3000])
 
 
 def test_transcribe_word_timestamps_end_to_end(micro_ml):
