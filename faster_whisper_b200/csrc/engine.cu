@@ -11,6 +11,7 @@
 #include <numeric>
 
 #include "model.h"
+#include "vad.h"
 
 namespace b2w {
 
@@ -1431,6 +1432,51 @@ static void check_row_table(const int32_t* rows, int R, int n_ctx, int slots, in
   }
 }
 
+
+// ---- Silero VAD ------------------------------------------------------------------------------------------------------
+// The weights b2w_vad_create takes: name, and shape (fp32 only).
+static const struct {
+  const char* name;
+  std::initializer_list<int64_t> shape;
+} kVadTensors[] = {
+    {"basis", {258, 256}},           {"conv0.weight", {128, 129, 3}}, {"conv0.bias", {128}}, {"conv1.weight", {64, 128, 3}},
+    {"conv1.bias", {64}},            {"conv2.weight", {64, 64, 3}},   {"conv2.bias", {64}},  {"conv3.weight", {128, 64, 3}},
+    {"conv3.bias", {128}},           {"lstm.w_ih", {512, 128}},       {"lstm.w_hh", {512, 128}}, {"lstm.bias", {512}},
+    {"decoder.weight", {128}},       {"decoder.bias", {1}},
+};
+
+struct b2w_vad {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  std::mutex mu;
+  ScratchBufs weights;        // every weight buffer and the LSTM state
+  VadWeights w;
+  const float *w_hh = nullptr, *dec_w = nullptr, *dec_b = nullptr;
+  float* state = nullptr;     // h [128] then c [128], carried from block to block
+  int64_t block = 32768;      // windows per block; the buffers below take (512 + 512 + 128 + 1) floats = 4.6 KB per window
+  int64_t cap = 0;            // windows the block buffers hold
+  std::unique_ptr<ScratchBufs> bufs;
+  float *pcm = nullptr, *gx = nullptr, *H = nullptr, *probs = nullptr;
+  cudaEvent_t ev[4] = {};
+  double ms[3] = {0, 0, 0};   // last call: window kernel, recurrence, decoder
+  ~b2w_vad() {  // the buffers are freed after this body, once the stream has drained
+    cudaSetDevice(device);
+    if (stream) cudaStreamSynchronize(stream);
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+  }
+};
+
+// host fp32 [rows][cols] -> device [cols][rows]
+static float* vad_upload_t(ScratchBufs& sb, const b2w_tensor& t, int64_t rows, int64_t cols) {
+  const float* src = static_cast<const float*>(t.data);
+  std::vector<float> h((size_t)(rows * cols));
+  for (int64_t r = 0; r < rows; ++r)
+    for (int64_t c = 0; c < cols; ++c) h[(size_t)(c * rows + r)] = src[r * cols + c];
+  return sb.put<float>(h.data(), h.size());
+}
+
 extern "C" {
 
 const char* b2w_last_error(void) { return g_last_error.c_str(); }
@@ -2194,6 +2240,111 @@ int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts
                                  cudaMemcpyDeviceToHost, s));
       B2W_CUDA(cudaStreamSynchronize(s));  // rows / anc are rewritten for the next step
     }
+  });
+}
+
+int b2w_vad_create(int32_t device, const b2w_tensor* tensors, int32_t n_tensors, b2w_vad** out) {
+  return guarded([&] {
+    B2W_CHECK(tensors && out && n_tensors >= 0, "null argument");
+    TensorTable tt{tensors, n_tensors};
+    for (const auto& spec : kVadTensors) {
+      const b2w_tensor& t = tt.get(spec.name);
+      B2W_CHECK(t.data && t.dtype == B2W_F32, "VAD weights must be float32");
+      expect_shape(t, spec.shape);
+    }
+    require_hopper(device);
+    DeviceGuard g(device);
+    std::unique_ptr<b2w_vad> v(new b2w_vad);
+    v->device = device;
+    B2W_CUDA(cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : v->ev) B2W_CUDA(cudaEventCreate(&e));
+    vad_configure();
+    ScratchBufs& sb = v->weights;
+    auto raw = [&](const char* name) { const b2w_tensor& t = tt.get(name); return sb.put<float>(t.data, (size_t)numel(t)); };
+    v->w.basis_t = vad_upload_t(sb, tt.get("basis"), 258, 256);
+    const int cout[4] = {128, 64, 64, 128}, cin[4] = {129, 128, 64, 64};
+    for (int i = 0; i < 4; ++i) {
+      const std::string p = "conv" + std::to_string(i);
+      v->w.conv_t[i] = vad_upload_t(sb, tt.get(p + ".weight"), cout[i], (int64_t)cin[i] * 3);
+      v->w.conv_b[i] = raw((p + ".bias").c_str());
+    }
+    v->w.w_ih_t = vad_upload_t(sb, tt.get("lstm.w_ih"), 512, 128);
+    v->w.b_gates = raw("lstm.bias");
+    v->w_hh = raw("lstm.w_hh");
+    v->dec_w = raw("decoder.weight");
+    v->dec_b = raw("decoder.bias");
+    v->state = sb.put<float>(nullptr, 0, 256);
+    *out = v.release();
+  });
+}
+
+void b2w_vad_destroy(b2w_vad* v) { delete v; }
+
+int b2w_vad_set_block(b2w_vad* v, int64_t windows) {
+  return guarded([&] {
+    B2W_CHECK(windows >= 1 && windows <= (1 << 24), "windows per block must be in 1..2^24");
+    B2W_CHECK(v, "null VAD handle");
+    std::lock_guard<std::mutex> lk(v->mu);
+    v->block = windows;
+  });
+}
+
+int b2w_vad_probs(b2w_vad* v, const float* pcm, int64_t n_samples, float* probs_out, int64_t capacity) {
+  return guarded([&] {
+    B2W_CHECK(pcm && probs_out, "null argument");
+    B2W_CHECK(n_samples > 0 && n_samples % 512 == 0, "the number of samples must be a positive multiple of 512");
+    const int64_t N = n_samples / 512;
+    B2W_CHECK(capacity >= N, "output buffer too small: one probability per 512 samples");
+    B2W_CHECK(v, "null VAD handle");
+    std::lock_guard<std::mutex> lk(v->mu);
+    DeviceGuard g(v->device);
+    cudaStream_t s = v->stream;
+    const int64_t nb_max = std::min(v->block, N);
+    if (v->cap < nb_max) {
+      v->bufs.reset();
+      v->cap = 0;
+      std::unique_ptr<ScratchBufs> b(new ScratchBufs);
+      v->pcm = b->alloc<float>((size_t)(64 + 512 * nb_max));
+      v->gx = b->alloc<float>((size_t)(512 * nb_max));
+      v->H = b->alloc<float>((size_t)(128 * nb_max));
+      v->probs = b->alloc<float>((size_t)nb_max);
+      v->bufs = std::move(b);
+      v->cap = nb_max;
+    }
+    B2W_CUDA(cudaMemsetAsync(v->state, 0, 256 * sizeof(float), s));
+    for (double& m : v->ms) m = 0;
+    for (int64_t n0 = 0; n0 < N; n0 += nb_max) {
+      const int nb = (int)std::min(nb_max, N - n0);
+      // the 64 samples before the block (zeros before the audio), then the block
+      if (n0 == 0) {
+        B2W_CUDA(cudaMemsetAsync(v->pcm, 0, 64 * sizeof(float), s));
+        B2W_CUDA(cudaMemcpyAsync(v->pcm + 64, pcm, (size_t)nb * 512 * 4, cudaMemcpyHostToDevice, s));
+      } else {
+        B2W_CUDA(cudaMemcpyAsync(v->pcm, pcm + n0 * 512 - 64, (64 + (size_t)nb * 512) * 4, cudaMemcpyHostToDevice, s));
+      }
+      B2W_CUDA(cudaEventRecord(v->ev[0], s));
+      vad_windows(v->w, v->pcm, nb, n0 + nb == N, v->gx, s);
+      B2W_CUDA(cudaEventRecord(v->ev[1], s));
+      vad_recurrence(v->w_hh, v->gx, nb, v->state, v->state + 128, v->H, s);
+      B2W_CUDA(cudaEventRecord(v->ev[2], s));
+      vad_decoder(v->H, v->dec_w, v->dec_b, nb, v->probs, s);
+      B2W_CUDA(cudaEventRecord(v->ev[3], s));
+      B2W_CUDA(cudaMemcpyAsync(probs_out + n0, v->probs, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+      B2W_CUDA(cudaStreamSynchronize(s));
+      for (int i = 0; i < 3; ++i) {
+        float ms = 0.f;
+        B2W_CUDA(cudaEventElapsedTime(&ms, v->ev[i], v->ev[i + 1]));
+        v->ms[i] += ms;
+      }
+    }
+  });
+}
+
+int b2w_vad_timing(b2w_vad* v, double ms_out[3]) {
+  return guarded([&] {
+    B2W_CHECK(v && ms_out, "null argument");
+    std::lock_guard<std::mutex> lk(v->mu);
+    for (int i = 0; i < 3; ++i) ms_out[i] = v->ms[i];
   });
 }
 

@@ -87,7 +87,7 @@ ABI_SYMBOLS = (
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
     "b2w_detect_language", "b2w_align", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
-    "b2w_debug_step_logits",
+    "b2w_debug_step_logits", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
 )
 
 
@@ -147,6 +147,12 @@ def load_library():
         lib.b2w_debug_fetch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
         lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                               C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.b2w_vad_create.argtypes = [C.c_int32, C.POINTER(_Tensor), C.c_int32, C.POINTER(C.c_void_p)]
+        lib.b2w_vad_destroy.argtypes = [C.c_void_p]
+        lib.b2w_vad_destroy.restype = None
+        lib.b2w_vad_probs.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        lib.b2w_vad_set_block.argtypes = [C.c_void_p, C.c_int64]
+        lib.b2w_vad_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         if lib.b2w_abi_version() != 1:
             raise RuntimeError("libb200whisper ABI version mismatch")
         _lib = lib
@@ -653,6 +659,48 @@ class Whisper:
         with rep.lock:
             _check(rep._lib.b2w_debug_fetch(rep.handle, int(which), _ptr(out), int(n)))
         return out
+
+
+class SileroVad:
+    """The Silero VAD v6 network on one GPU (``b2w_vad_*``): ``probs(pcm)`` returns one speech probability per 512-sample window.
+    ``weights`` are the arrays ``silero.load_weights`` returns (names and shapes in include/b200whisper.h)."""
+
+    def __init__(self, weights: Dict[str, np.ndarray], device: int = 0, block_windows: Optional[int] = None):
+        lib = load_library()
+        keep, tensors = [], []
+        for name, arr in weights.items():
+            arr = np.ascontiguousarray(arr, dtype=np.float32)
+            keep.append(arr)
+            t = _Tensor(name=name.encode(), data=arr.ctypes.data, dtype=0, ndim=arr.ndim)
+            for i, n in enumerate(arr.shape[:4]):
+                t.shape[i] = n
+            tensors.append(t)
+        arr_t = (_Tensor * max(len(tensors), 1))(*tensors)
+        h = C.c_void_p()
+        _check(lib.b2w_vad_create(device, arr_t, len(tensors), C.byref(h)))
+        self._lib, self._h = lib, h
+        if block_windows is not None:
+            _check(lib.b2w_vad_set_block(h, block_windows))
+
+    def probs(self, pcm: np.ndarray) -> np.ndarray:
+        x = np.ascontiguousarray(pcm, dtype=np.float32)
+        out = np.empty(x.shape[0] // 512, np.float32)
+        _check(self._lib.b2w_vad_probs(self._h, _ptr(x), x.shape[0], _ptr(out), out.shape[0]))
+        return out
+
+    def timing(self) -> Dict[str, float]:
+        """Device milliseconds of the last ``probs`` call per kernel."""
+        ms = (C.c_double * 3)()
+        _check(self._lib.b2w_vad_timing(self._h, ms))
+        return dict(zip(("window", "recurrence", "decoder"), ms))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b2w_vad_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
 
 
 class models:  # namespace shim so `ctranslate2.models.Whisper` style access works on this module

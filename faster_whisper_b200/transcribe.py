@@ -336,7 +336,7 @@ class BatchedInferencePipeline:
                 elif isinstance(vad_parameters, dict):
                     vad_parameters = VadOptions(**{**{k: v for k, v in vad_parameters.items() if k != "max_speech_duration_s"},
                                                    "max_speech_duration_s": chunk_length})
-                clip_timestamps = get_speech_timestamps(audio, vad_parameters)
+                clip_timestamps = get_speech_timestamps(audio, vad_parameters, device_index=model.model.device_index[0])
             elif duration < chunk_length:
                 clip_timestamps = [{"start": 0, "end": audio.shape[0]}]
             else:
@@ -576,7 +576,7 @@ class WhisperModel:
                 vad_parameters = VadOptions()
             elif isinstance(vad_parameters, dict):
                 vad_parameters = VadOptions(**vad_parameters)
-            speech_chunks = get_speech_timestamps(audio, vad_parameters)
+            speech_chunks = get_speech_timestamps(audio, vad_parameters, device_index=self.model.device_index[0])
             pieces, _ = collect_chunks(audio, speech_chunks)
             audio = np.concatenate(pieces, axis=0)
             duration_after_vad = audio.shape[0] / sr
@@ -969,7 +969,7 @@ class WhisperModel:
         fe = self.feature_extractor
         if audio is not None:
             if vad_filter:
-                spans = get_speech_timestamps(audio, vad_parameters)
+                spans = get_speech_timestamps(audio, vad_parameters, device_index=self.model.device_index[0])
                 pieces, _ = collect_chunks(audio, spans)
                 audio = np.concatenate(pieces, axis=0)
             features = fe(audio[: language_detection_segments * fe.n_samples])

@@ -1,15 +1,15 @@
 """Voice-activity chunking (``faster_whisper/vad.py``).
 
-The Silero VAD network itself (ONNX, CPU LSTM) is outside the accelerated path (SURVEY.md §2.1 row 6).  The speech
-probabilities come from a pluggable model: by default the Silero ONNX asset through onnxruntime, exactly as the reference
-loads it (``vad.py:286-351``) — neither ships with this engine, so ``get_speech_timestamps`` raises the reference's
-RuntimeError unless onnxruntime is importable and ``B2W_SILERO_VAD`` (or ``assets/silero_vad_v6.onnx`` next to this file)
-names the model; ``set_vad_model`` installs any other ``audio -> probabilities per 512-sample window`` callable.
+The speech probabilities come from the Silero VAD v6 network, one per 512-sample window.  ``get_vad_model()`` loads it from
+``B2W_SILERO_VAD`` or ``assets/silero_vad_v6.onnx`` next to this file, as the reference loads its asset (``vad.py:286-351``):
+through onnxruntime on the CPU when onnxruntime is importable (``SileroVADModel``, exactly the reference's session), otherwise
+on the GPU (``SileroGpuVAD``: the ONNX file is read by ``silero.py`` without onnxruntime, and the network runs as the CUDA
+kernels of ``csrc/vad.cu``, fp32 throughout, checked against a float64 restatement).  A missing model file raises RuntimeError;
+``set_vad_model`` installs any other ``audio -> probabilities per 512-sample window`` callable.
 Everything around the network — the hysteresis segmenter (``vad.py:44-183``), ``collect_chunks`` and ``SpeechTimestampsMap``
 (``vad.py:186-285``) — is implemented here and checked against the reference's functions on the same probabilities
 (tests/test_dropin.py).
 """
-
 from __future__ import annotations
 
 import bisect
@@ -31,21 +31,36 @@ class VadOptions:
 
 
 _WINDOW = 512  # samples per probability (Silero v5+/v6 at 16 kHz)
-_vad_model = None
+_vad_model = None   # installed by set_vad_model
+_silero: dict = {}  # default Silero models by (path, None for onnxruntime on the CPU or the GPU index)
 
 
 def set_vad_model(model) -> None:
     """Installs the speech-probability model: ``model(padded_audio) -> array of one probability per 512-sample window``
-    (None restores the default Silero/onnxruntime loader)."""
+    (None restores the default Silero loader)."""
     global _vad_model
     _vad_model = model
 
 
-def get_vad_model():
-    global _vad_model
-    if _vad_model is None:
-        _vad_model = SileroVADModel(os.environ.get("B2W_SILERO_VAD") or os.path.join(os.path.dirname(__file__), "assets", "silero_vad_v6.onnx"))
-    return _vad_model
+def get_vad_model(device_index: int = 0):
+    """The installed model, else Silero: through onnxruntime when it is importable, otherwise on GPU ``device_index``
+    (the transcription model's first device)."""
+    if _vad_model is not None:
+        return _vad_model
+    path = os.environ.get("B2W_SILERO_VAD") or os.path.join(os.path.dirname(__file__), "assets", "silero_vad_v6.onnx")
+    try:
+        import onnxruntime  # noqa: F401
+    except ImportError:
+        key, make = (path, device_index), lambda: SileroGpuVAD(path, device=device_index)
+    else:
+        key, make = (path, None), lambda: SileroVADModel(path)
+    if key not in _silero:
+        _silero[key] = make()
+    return _silero[key]
+
+
+def _missing_model(path: str) -> RuntimeError:
+    return RuntimeError(f"Silero VAD model not found at {path}; set B2W_SILERO_VAD or use vad_filter=False with clip_timestamps")
 
 
 class SileroVADModel:
@@ -57,7 +72,7 @@ class SileroVADModel:
         except ImportError as e:
             raise RuntimeError("Applying the VAD filter requires the onnxruntime package") from e
         if not os.path.isfile(path):
-            raise RuntimeError(f"Silero VAD model not found at {path}; set B2W_SILERO_VAD or use vad_filter=False with clip_timestamps")
+            raise _missing_model(path)
         opts = onnxruntime.SessionOptions()
         opts.inter_op_num_threads = 1
         opts.intra_op_num_threads = 1
@@ -79,6 +94,23 @@ class SileroVADModel:
             out, h, c = self.session.run(None, {"input": x[lo : lo + 10000], "h": h, "c": c})
             outs.append(out)
         return np.concatenate(outs, axis=0)
+
+
+class SileroGpuVAD:
+    """The Silero VAD ONNX graph on the GPU (csrc/vad.cu), with SileroVADModel's contract: padded audio in, one probability
+    per 512-sample window out (same window context, same zeroed tail of the last window, LSTM state carried through)."""
+
+    def __init__(self, path: str, device: int = 0, block_windows: Optional[int] = None):
+        if not os.path.isfile(path):
+            raise _missing_model(path)
+        from . import engine, silero
+
+        self.model = engine.SileroVad(silero.load_weights(path), device=device, block_windows=block_windows)
+
+    def __call__(self, audio: np.ndarray, num_samples: int = _WINDOW, context: int = 64) -> np.ndarray:
+        assert audio.ndim == 1 and audio.shape[0] % num_samples == 0
+        assert num_samples == _WINDOW and context == 64, "the network takes 512-sample windows after 64 context samples"
+        return self.model.probs(audio)
 
 
 class _Segmenter:
@@ -151,11 +183,13 @@ class _Segmenter:
         return self.out
 
 
-def get_speech_timestamps(audio: np.ndarray, vad_options: Optional[VadOptions] = None, sampling_rate: int = 16000, **kwargs) -> List[dict]:
-    """Speech spans ``[{"start": sample, "end": sample}, ...]`` (``vad.py:44-183``)."""
+def get_speech_timestamps(audio: np.ndarray, vad_options: Optional[VadOptions] = None, sampling_rate: int = 16000,
+                          device_index: int = 0, **kwargs) -> List[dict]:
+    """Speech spans ``[{"start": sample, "end": sample}, ...]`` (``vad.py:44-183``); ``device_index``: the GPU of the default
+    Silero model when it runs on the GPU."""
     o = vad_options if vad_options is not None else VadOptions(**kwargs)
     n = len(audio)
-    model = get_vad_model()
+    model = get_vad_model(device_index)
     probs = model(np.pad(audio, (0, _WINDOW - audio.shape[0] % _WINDOW)))
     seg = _Segmenter(o, sampling_rate)
     for i, p in enumerate(probs):

@@ -144,6 +144,26 @@ int b2w_align(b2w_model* m, b2w_encoded* e, int32_t batch_index, const int32_t* 
  * (layer, head) pairs; n_pairs = 0 restores the default (every head of the last half of the decoder layers). */
 int b2w_model_set_alignment_heads(b2w_model* m, const int32_t* layer_head_pairs, int32_t n_pairs);
 
+/* ---- voice activity -----------------------------------------------------------------------------
+ * The Silero VAD v6 network (16 kHz) of vad.py's SileroVADModel on the GPU, fp32 throughout.  Weights (float32, names and shapes
+ * as faster_whisper_b200/silero.py reads them from the ONNX file): basis [258][256], conv{0..3}.weight [out][in][3] and .bias
+ * [out] (129->128, 128->64, 64->64, 64->128), lstm.w_ih [512][128], lstm.w_hh [512][128], lstm.bias [512] (b_ih + b_hh; gate
+ * blocks i, o, f, c), decoder.weight [128], decoder.bias [1].  Every name and shape is checked before any device work.  A handle
+ * owns its stream and buffers and serialises its calls. */
+typedef struct b2w_vad b2w_vad;
+int b2w_vad_create(int32_t device, const b2w_tensor* weights, int32_t n_weights, b2w_vad** out);
+void b2w_vad_destroy(b2w_vad* vad);
+/* One speech probability per 512-sample window of host PCM (n_samples a positive multiple of 512): probs_out[n_samples / 512],
+ * capacity in floats.  As SileroVADModel: window n sees the last 64 samples of window n-1 first (zeros for n = 0), and the
+ * last window's own final 64 samples count as zero.  The LSTM state starts at zero; the audio runs through in blocks of windows
+ * (b2w_vad_set_block) with the state carried on the device, and the result does not depend on the block size. */
+int b2w_vad_probs(b2w_vad* vad, const float* pcm, int64_t n_samples, float* probs_out, int64_t capacity);
+/* Windows per block (default 32768, about 17.5 min of audio).  The block buffers take 4.6 KB of device memory per window (PCM,
+ * LSTM inputs, hidden states, probabilities): 151 MB at the default. */
+int b2w_vad_set_block(b2w_vad* vad, int64_t windows);
+/* Device time of the last b2w_vad_probs call in milliseconds: window kernel, recurrence, decoder (CUDA events). */
+int b2w_vad_timing(b2w_vad* vad, double ms_out[3]);
+
 /* ---- measurement --------------------------------------------------------------------------------
  * CUDA-event stage timers accumulated since the last reset (the roofline report in bench.py). */
 enum { B2W_T_MEL = 0, B2W_T_ENCODER = 1, B2W_T_CROSSKV = 2, B2W_T_PREFILL = 3, B2W_T_DECODE = 4,
