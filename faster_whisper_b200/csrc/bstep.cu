@@ -3,7 +3,7 @@
 // At 80 rows a decode step is a chain of skinny GEMMs [R x K] x [K x N] (3-13 MB of weights each), 1600 self-attention
 // (row, head) tasks over the paged self-KV cache and 2240 beam-shared cross-attention tasks that stream 3.9 GB of cross-K/V.
 // As separate launches that is ~260 graph nodes; here one CTA per SM stays resident and walks
-//   embed | L x { QKV, self-attn, out-proj, cross-q, cross-attn, cross-out, FFN1, GELU, FFN2 } | final LN | logits
+//   embed | L x { QKV, self-attn, out-proj, cross-q, cross-attn, cross-out, FFN1 + GELU, FFN2 } | final LN | logits
 // separated by grid barriers.  What shapes it (DESIGN.md §4):
 //   * L2 -> SM bandwidth is only a small multiple of HBM bandwidth, so no phase may broadcast the [R x K] activations to
 //     every CTA (205 KB x 132 per phase would cost more than the weights).  Every GEMM is therefore split over output
@@ -14,11 +14,13 @@
 //     warpgroups multiplies its 64 channels of every atom against the staged activations;
 //   * split-K partial sums meet in L2 in a fixed order, so that a step computes the same bits every run: each CTA stores its
 //     [R x 128] fp32 partial tile with one bulk copy into its own slot, the CTAs of an n-block meet at a counter, and each then
-//     sums a slice of the rows over the group's partials in CTA order;
+//     sums a slice of the rows over the group's partials in CTA order.  The QKV and cross-q partials skip the meet: the attention
+//     phase after the next grid barrier sums them itself, in the same order, while it loads its q / k / v;
 //   * since no CTA ever sees a whole row of a GEMM output, everything that needs one is deferred to the consumer: the
 //     LayerNorm of a residual-stream input is applied algebraically, y = rstd (W x - mean rowsum(W)) + b, with sum(x) and
-//     sum(x^2) taken from the staged fp16 tiles (per k-atom, by the CTAs of n-block 0, summed in k order in the reduction); biases of
-//     q/k/v/cross-q/hidden are added by the consumer; GELU gets its own (cheap, rolled) phase so that it is evaluated once per element;
+//     sum(x^2) taken from the staged fp16 tiles (per k-atom, by the CTAs of n-block 0, summed in k order by the consumer); biases of
+//     q/k/v/cross-q/hidden are added by the consumer; FFN1's reduction sums every hidden element exactly once, so it applies
+//     LayerNorm, bias and GELU there;
 //   * a weight-producer thread keeps a 5-slot ring of atoms full across phase boundaries, a K/V-producer thread double
 //     buffers the cross-attention tiles; eight compute warps do the rest;
 //   * the phase code runs ONCE per phase on eight warps (two per scheduler) and the ~110 KB of it cycle through a 32 KB instruction
@@ -103,32 +105,32 @@ struct BsShared {
 };
 
 // ---- phase numbering -------------------------------------------------------------------------------------------------------
-// grid phase index: 0 embed; 1 + 9 l + {0 qkv, 1 self, 2 out, 3 cross_q, 4 cross, 5 cross_out, 6 ffn1, 7 gelu, 8 ffn2}; 1 + 9 L final LN; 2 + 9 L logits
+// grid phase index: 0 embed; 1 + 8 l + {0 qkv, 1 self, 2 out, 3 cross_q, 4 cross, 5 cross_out, 6 ffn1 (+ GELU), 7 ffn2}; 1 + 8 L final LN;
+// 2 + 8 L logits
 __device__ __forceinline__ bool bs_enabled(const BStepArgs& a, int phase) { return a.stop_phase <= 0 || phase < a.stop_phase; }
 // GEMM sequence s = 6 l + j (j: qkv, out, cross_q, cross_out, ffn1, ffn2) -> grid phase
 __device__ __forceinline__ int bs_gemm_phase_index(int s) {
   const int l = s / 6, j = s - 6 * l;
-  const int ph = j == 0 ? 0 : (j == 1 ? 2 : (j == 2 ? 3 : (j == 3 ? 5 : (j == 4 ? 6 : 8))));
-  return 1 + 9 * l + ph;
+  const int ph = j == 0 ? 0 : (j == 1 ? 2 : (j == 2 ? 3 : (j == 3 ? 5 : (j == 4 ? 6 : 7))));
+  return 1 + 8 * l + ph;
 }
-// Atoms of GEMM s owned by this CTA.  The CTAs are dealt out to the n-blocks (as evenly as the counts allow) and the CTAs of an
-// n-block split its K atoms among themselves, so a CTA's run never crosses an n-block: one accumulator, one epilogue, one partial
-// tile per phase.  Needs at least as many CTAs as n-blocks (bstep_supported).
+// The CTAs bs_split deals to n-block nb: the first one, g0, and how many of them own atoms, gn.  The n-blocks get G / NB CTAs each
+// and the first G % NB of them one more; a group never has more CTAs than k-atoms, so every CTA counted in it has work.
+__host__ __device__ __forceinline__ void bs_group(int NB, int KA, int G, int nb, int& g0, int& gn) {
+  const int base = G / NB, extra = G - base * NB;
+  g0 = nb * base + (nb < extra ? nb : extra);
+  gn = nb < extra ? base + 1 : base;
+  if (gn > KA) gn = KA;
+}
+// Atoms of GEMM s owned by this CTA.  The CTAs are dealt out to the n-blocks (bs_group) and the CTAs of an n-block split its K atoms
+// among themselves, so a CTA's run never crosses an n-block: one accumulator, one epilogue, one partial tile per phase.  Needs at
+// least as many CTAs as n-blocks (bstep_supported).
 __host__ __device__ __forceinline__ void bs_split(int NB, int KA, int c, int G, int& a0, int& a1, int& idx, int& cnt) {
   const int base = G / NB, extra = G - base * NB;
-  int nb;
-  if (c < extra * (base + 1)) {
-    nb = c / (base + 1);
-    idx = c - nb * (base + 1);
-    cnt = base + 1;
-  } else {
-    const int c2 = c - extra * (base + 1);
-    nb = extra + c2 / base;
-    idx = c2 - (c2 / base) * base;
-    cnt = base;
-  }
-  // at most one CTA per k-atom: every CTA counted in a group has work, so all of them reach the group's meeting point
-  if (cnt > KA) cnt = KA;
+  const int nb = c < extra * (base + 1) ? c / (base + 1) : extra + (c - extra * (base + 1)) / base;
+  int g0;
+  bs_group(NB, KA, G, nb, g0, cnt);
+  idx = c - g0;
   if (idx >= cnt) {
     a0 = a1 = nb * KA;
     return;
@@ -190,7 +192,7 @@ __device__ __noinline__ void bs_weight_producer(const BStepArgs& a, BsShared& sh
 #pragma unroll 1
     for (int at = r.a0; at < r.a1; ++at) push(base, (size_t)at);
   }
-  if (!bs_enabled(a, 2 + 9 * a.L)) return;
+  if (!bs_enabled(a, 2 + 8 * a.L)) return;
   int nhalves, Rh, NPh;
   bs_logit_plan(a.R, a.d, kBsKvBytes + a.u_bytes, nhalves, Rh, NPh);
   const int groups = gridDim.x / nhalves, grp = blockIdx.x / nhalves;
@@ -237,7 +239,7 @@ __device__ __noinline__ void bs_kv_producer(const BStepArgs& a, BsShared& sh, un
   const int n_even = (nt + 1) >> 1, n_odd = nt >> 1;
 #pragma unroll 1
   for (int l = 0; l < a.L; ++l) {
-    if (!bs_enabled(a, 1 + 9 * l + 4)) return;
+    if (!bs_enabled(a, 1 + 8 * l + 4)) return;
 #pragma unroll 1
     for (int k = 0; k < nt; ++k) {
       const int buf = k & 1;
@@ -256,10 +258,48 @@ __device__ __noinline__ void bs_kv_producer(const BStepArgs& a, BsShared& sh, un
 // ---- compute-warp phase functions ------------------------------------------------------------------------------------------
 // (all out of line: the phase loop of the kernel body must not spill — with 220 KB of shared memory the L1 is ~28 KB and local
 // memory lives in L2 for all practical purposes)
-// The fp32 GEMM outputs (x, qkv32, cq32, h32) are stored n-block-major: element (row r, channel n) lives at
-// ((n >> 7) * R + r) * 128 + (n & 127), so that the [R x 128] output tile of a GEMM segment is ONE contiguous block, like the
-// partial tiles the CTAs store with one bulk copy each (bulk instructions are warp-uniform: one per row would serialise 80 issues).
+// The fp32 residual stream x is stored n-block-major: element (row r, channel n) lives at ((n >> 7) * R + r) * 128 + (n & 127), so
+// that the [R x 128] output tile of a GEMM segment is ONE contiguous block, like the partial tiles the CTAs store with one bulk copy
+// each into gpart (bulk instructions are warp-uniform: one per row would serialise 80 issues).
 __device__ __forceinline__ long long bs_bidx(int R, int r, int n) { return ((long long)(n >> 7) * R + r) * 128 + (n & 127); }
+
+__device__ __forceinline__ float2 bs_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float4 bs_add(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+// p[0] + p[s] + ... + p[(n - 1) s], added in exactly that order, with up to B loads in flight.  Every split-K sum and every sum of the
+// per-k-atom row statistics goes through here, whichever phase does it, so a value is the same bits wherever it is computed.
+template <int B, typename T>
+__device__ __forceinline__ T bs_ordered_sum(const T* p, long long s, int n) {
+  T t = __ldcg(p);
+#pragma unroll 1
+  for (int k0 = 1; k0 < n; k0 += B) {
+#pragma unroll
+    for (int i = 0; i < B; ++i) {  // loads of the tail re-read the last term: unconditional loads can all be in flight at once
+      const int k = k0 + i < n ? k0 + i : n - 1;
+      const T u = __ldcg(p + k * s);
+      if (k0 + i < n) t = bs_add(t, u);
+    }
+  }
+  return t;
+}
+
+// The split-K sum of GEMM output (row r, channel n), from the partial tiles the CTAs of n-block n >> 7 left in gpart (CTA order).
+// NB / KA: n-blocks / k-atoms of the GEMM; T = float2 / float4: that many consecutive channels.
+template <typename T>
+__device__ __forceinline__ T bs_part_sum(const BStepArgs& a, int NB, int KA, int r, int n) {
+  int g0, gn;
+  bs_group(NB, KA, (int)gridDim.x, n >> 7, g0, gn);
+  constexpr int P = sizeof(T) / sizeof(float);
+  return bs_ordered_sum<8>(reinterpret_cast<const T*>(a.gpart + ((long long)g0 * a.R + r) * 128 + (n & 127)), (long long)a.R * (128 / P), gn);
+}
+
+// sum(x), sum(x^2) of row r of a LayerNorm input: the per-k-atom partials bs_tile_stats left in stpart, in k order (KA <= 20)
+__device__ __forceinline__ float2 bs_row_sums(const BStepArgs& a, int r) {
+  return bs_ordered_sum<20>(reinterpret_cast<const float2*>(a.stpart) + r, a.R, a.d >> 6);
+}
+__device__ __forceinline__ void bs_row_norm(float2 s, int d, float& mean, float& rstd) {
+  mean = s.x / d;
+  rstd = rsqrtf(fmaxf(s.y / d - mean * mean, 0.f) + 1e-5f);
+}
 
 // embed: x = tok_emb[token] + pos_emb[pos] (CTA r owns row r)
 __device__ __noinline__ void bs_embed_phase(const BStepArgs& a, BsShared& sh) {
@@ -271,12 +311,6 @@ __device__ __noinline__ void bs_embed_phase(const BStepArgs& a, BsShared& sh) {
     for (int i = threadIdx.x; i < d; i += kBsThreads)
       __stcg(a.x + bs_bidx(a.R, r, i), __half2float(a.tok_emb[(long long)tok * d + i]) + a.pos_emb[(long long)pos * d + i]);
   }
-}
-
-__device__ __forceinline__ void bs_row_stats(const float* st, int r, int d, float& mean, float& rstd) {
-  const float2 s = __ldcg(reinterpret_cast<const float2*>(st) + r);
-  mean = s.x / d;
-  rstd = rsqrtf(fmaxf(s.y / d - mean * mean, 0.f) + 1e-5f);
 }
 
 // ---- staging: this CTA's activation slices as wgmma B tiles --------------------------------------------------------
@@ -371,8 +405,8 @@ __device__ __noinline__ void bs_stage_h(const __half* __restrict__ src, int ld, 
 }
 
 // sum(x), sum(x^2) of the rows of a residual-stream input, from the staged fp16 tiles (i.e. of exactly the values the GEMM multiplies),
-// one partial per k-atom: st[ka][row][2].  The CTAs of n-block 0 stage every k-atom exactly once, so they alone write them; they also
-// sum them in k order (bs_gemm_mma).
+// one partial per k-atom: st[ka][row][2].  The CTAs of n-block 0 stage every k-atom exactly once, so they alone write them; whoever
+// applies the LayerNorm sums them in k order (bs_row_sums).
 __device__ __noinline__ void bs_tile_stats(float* st, int R, int r0, int Rw, int NPw, int natoms, int ka00, const unsigned char* xs) {
   const int tid = threadIdx.x, c = tid & 7, r_lo = tid >> 3;
 #pragma unroll 1
@@ -481,14 +515,18 @@ __device__ __forceinline__ void bs_stage_acc(const float (&acc)[NP / 2], float* 
   }
 }
 
-// The products of one GEMM run (one n-block segment, bstep_supported) and the fixed-order reduction of the n-block's partial tiles:
-// out = sum of the group's partials in CTA order (+ the residual already in out when `resid`).  `st` (LayerNorm-consuming GEMMs):
-// the CTAs of n-block 0 also sum the per-atom row statistics in k order.  A leaf function per row count: the accumulator
-// registers stay out of the phase code's own live ranges.
+// The products of one GEMM run (one n-block segment, bstep_supported) into this CTA's partial tile in gpart, then, for every GEMM but
+// QKV and cross-q, the fixed-order reduction of the n-block's partial tiles: the CTAs of the n-block meet at a counter and each sums a
+// slice of the rows over the group's partials in CTA order.  The residual GEMMs (out-proj, cross-out, FFN2) add the sum into x; FFN1
+// applies the deferred LayerNorm, its bias and GELU and writes h16.  The QKV and cross-q partials are left for the attention phases,
+// which sum them (and the row statistics) the same way while loading.  A leaf function per row count: the accumulator registers
+// stay out of the phase code's own live ranges.
 template <int NP>
 __device__ __noinline__ void bs_gemm_mma(const BStepArgs& a, BsShared& sh, const BsRange& rg, int s, unsigned char* U, unsigned char* ring,
-                                         float* out, int N, const float* bias, const float* scale, bool resid, float* st) {
+                                         int N, const float* bias, const float* scale) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, R = a.R;
+  const int l = s / 6, j = s - 6 * l;
+  const bool reduce = j != 0 && j != 2, gelu = j == 4;
   float acc[NP / 2];
 #pragma unroll
   for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
@@ -517,46 +555,52 @@ __device__ __noinline__ void bs_gemm_mma(const BStepArgs& a, BsShared& sh, const
     bs_bulk_store(a.gpart + (long long)blockIdx.x * R * 128, stg, (uint32_t)R * 512u);
     bs_bulk_commit();
     bs_bulk_wait_all();
-    bs_fence_async_all();
-    unsigned* cnt = a.bar + 64 + (s % 6) * 64 + rg.nb0;  // counts up through the layers: the same groups meet once per layer
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(cnt), "r"(1u) : "memory");
-    const unsigned target = (unsigned)((s / 6 + 1) * rg.gn);
-    unsigned v;
-    do {
-      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(cnt) : "memory");
-    } while (v < target);
-    asm volatile("fence.acq_rel.gpu;" ::: "memory");  // acquire: the group's partial tiles and statistics are read after this
+    bs_fence_async_all();  // QKV / cross-q: the grid barrier's release publishes the partial tile
+    if (reduce) {
+      unsigned* cnt = a.bar + 64 + j * 64;  // [n-block]; counts up through the layers: the same groups meet once per layer
+      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(cnt + rg.nb0), "r"(1u) : "memory");
+      unsigned v;
+      do {
+        asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(cnt + rg.nb0) : "memory");
+      } while (v < (unsigned)((l + 1) * rg.gn));
+      if (gelu && rg.nb0 != 0) {  // the row statistics are complete once n-block 0's group has met (bs_tile_stats precedes its arrival)
+        int g00, gn0;
+        bs_group((N + 127) >> 7, rg.KA, (int)gridDim.x, 0, g00, gn0);
+        do {
+          asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(cnt) : "memory");
+        } while (v < (unsigned)((l + 1) * gn0));
+      }
+      asm volatile("fence.acq_rel.gpu;" ::: "memory");  // acquire: the group's partial tiles and statistics are read after this
+    }
   }
   bs_sync();
+  if (!reduce) return;
   const int r0 = R * rg.gi / rg.gn, r1 = R * (rg.gi + 1) / rg.gn;  // this CTA's rows of the sum
-  const float* p0 = a.gpart + (long long)rg.g0 * R * 128;
-  float* o = out + (long long)rg.nb0 * R * 128;
+  const float4* p0 = reinterpret_cast<const float4*>(a.gpart + (long long)rg.g0 * R * 128);
+  if (gelu) {  // h16 = GELU(rstd (h - mean rowsum(W1)) + b1): a warp per row, a thread keeps one column group of 4 channels
+    const int n = rg.nb0 * 128 + lane * 4;
+    const BLayer& lay = sh.lay[l];
+    const float4 ws = __ldg(reinterpret_cast<const float4*>(lay.wsum[2] + n)), bb = __ldg(reinterpret_cast<const float4*>(lay.bias[4] + n));
+#pragma unroll 1
+    for (int i = r0 * 32 + tid; i < r1 * 32; i += kBsThreads) {
+      const int r = i >> 5;
+      const float2 ss = bs_row_sums(a, r);
+      const float4 h = bs_ordered_sum<8>(p0 + i, (long long)R * 32, rg.gn);
+      if (rg.nb0 == 0 && lane == 0) __stcg(reinterpret_cast<float2*>(a.stats) + (long long)(3 * l + 2) * R + r, ss);
+      float mean, rstd;
+      bs_row_norm(ss, a.d, mean, rstd);
+      const float mr = mean * rstd;
+      const float y0 = gelu_erf(fmaf(rstd, h.x, fmaf(-mr, ws.x, bb.x))), y1 = gelu_erf(fmaf(rstd, h.y, fmaf(-mr, ws.y, bb.y)));
+      const float y2 = gelu_erf(fmaf(rstd, h.z, fmaf(-mr, ws.z, bb.z))), y3 = gelu_erf(fmaf(rstd, h.w, fmaf(-mr, ws.w, bb.w)));
+      *reinterpret_cast<uint2*>(a.h16 + (long long)r * N + n) = make_uint2(pack_half2(y0, y1), pack_half2(y2, y3));
+    }
+    return;
+  }
+  float4* o = reinterpret_cast<float4*>(a.x + (long long)rg.nb0 * R * 128);
 #pragma unroll 1
   for (int i = r0 * 32 + tid; i < r1 * 32; i += kBsThreads) {
-    float4 t = __ldcg(reinterpret_cast<const float4*>(p0) + i);
-#pragma unroll 1
-    for (int k = 1; k < rg.gn; ++k) {
-      const float4 u = __ldcg(reinterpret_cast<const float4*>(p0 + (long long)k * R * 128) + i);
-      t = make_float4(t.x + u.x, t.y + u.y, t.z + u.z, t.w + u.w);
-    }
-    if (resid) {
-      const float4 x = __ldcg(reinterpret_cast<const float4*>(o) + i);
-      t = make_float4(x.x + t.x, x.y + t.y, x.z + t.z, x.w + t.w);
-    }
-    __stcg(reinterpret_cast<float4*>(o) + i, t);
-  }
-  if (st && rg.nb0 == 0) {
-    const float2* sp = reinterpret_cast<const float2*>(a.stpart);
-#pragma unroll 1
-    for (int r = r0 + tid; r < r1; r += kBsThreads) {
-      float2 t = __ldcg(sp + r);
-#pragma unroll 1
-      for (int ka = 1; ka < rg.KA; ++ka) {
-        const float2 u = __ldcg(sp + (long long)ka * R + r);
-        t = make_float2(t.x + u.x, t.y + u.y);
-      }
-      __stcg(reinterpret_cast<float2*>(st) + r, t);
-    }
+    const float4 t = bs_ordered_sum<8>(p0 + i, (long long)R * 32, rg.gn);
+    __stcg(o + i, bs_add(__ldcg(o + i), t));
   }
 }
 
@@ -579,7 +623,6 @@ __device__ __noinline__ void bs_gemm_phase(const BStepArgs& a, BsShared& sh, int
       else bs_stage_h<3>(src, ld, 0, a.R, a.NP, natoms, rg.n0, rg.ka00, U);
     }
   }
-  float* out = j == 0 ? a.qkv32 : (j == 2 ? a.cq32 : (j == 4 ? a.h32 : a.x));
   const int N = j == 0 ? 3 * d : (j == 4 ? 4 * d : d);
   const float* bias = (j == 1 || j == 3 || j == 5) ? lay.bias[j] : nullptr;
   BS_TICK(0);
@@ -588,22 +631,20 @@ __device__ __noinline__ void bs_gemm_phase(const BStepArgs& a, BsShared& sh, int
   BS_TICK(4);
   const bool ln_input = j == 0 || j == 2 || j == 4;  // a residual-stream input: LayerNorm statistics of its rows (n-block 0's CTAs)
   if (ln_input && rg.nb0 == 0) bs_tile_stats(a.stpart, a.R, 0, a.R, a.NP, rg.a1 - rg.a0, rg.ka00, U);
-  float* st = ln_input ? a.stats + (long long)(3 * l + (j >> 1)) * a.R * 2 : nullptr;
-  const bool resid = !ln_input;  // out-proj, cross-out and FFN2 add into the residual stream
   BS_TICK(5);
   switch (a.NP) {
-    case 16: bs_gemm_mma<16>(a, sh, rg, s, U, ring, out, N, bias, lay.scale[j], resid, st); break;
-    case 32: bs_gemm_mma<32>(a, sh, rg, s, U, ring, out, N, bias, lay.scale[j], resid, st); break;
-    case 48: bs_gemm_mma<48>(a, sh, rg, s, U, ring, out, N, bias, lay.scale[j], resid, st); break;
-    case 64: bs_gemm_mma<64>(a, sh, rg, s, U, ring, out, N, bias, lay.scale[j], resid, st); break;
-    default: bs_gemm_mma<80>(a, sh, rg, s, U, ring, out, N, bias, lay.scale[j], resid, st); break;
+    case 16: bs_gemm_mma<16>(a, sh, rg, s, U, ring, N, bias, lay.scale[j]); break;
+    case 32: bs_gemm_mma<32>(a, sh, rg, s, U, ring, N, bias, lay.scale[j]); break;
+    case 48: bs_gemm_mma<48>(a, sh, rg, s, U, ring, N, bias, lay.scale[j]); break;
+    case 64: bs_gemm_mma<64>(a, sh, rg, s, U, ring, N, bias, lay.scale[j]); break;
+    default: bs_gemm_mma<80>(a, sh, rg, s, U, ring, N, bias, lay.scale[j]); break;
   }
   BS_TICK(2);
   BS_TICK_COUNT(j);
 }
 
-// Masked self-attention: one (row, head) task per warp.  q, k, v of the new token come from the raw QKV sums (deferred LayerNorm +
-// bias applied here); k and v are rounded to fp16 and written to the paged cache.  The history is gathered through the beam
+// Masked self-attention: one (row, head) task per warp.  q, k, v of the new token are summed here from the QKV GEMM's split-K partials
+// and per-k-atom row statistics (deferred LayerNorm + bias applied here); k and v are rounded to fp16 and written to the paged cache.  The history is gathered through the beam
 // ancestry table in blocks of 16 keys with an online softmax.  The K and V rows of a block are copied into the warp's own
 // shared-memory tile with cp.async — COALESCED: eight lanes copy the eight 16-byte chunks of one 128-byte row, so an instruction
 // touches 4 cache lines, not 32 — and double buffered: the copies of block b + 1 are in flight while block b is scored.  With only
@@ -616,7 +657,7 @@ __device__ __noinline__ void bs_self_attn_phase(const BStepArgs& a, BsShared& sh
   __half* qs = reinterpret_cast<__half*>(U + (size_t)kBsWarps * kBsSelfTile) + warp * 64;  // the task's query, fp16, pre-scaled by 1/8
   const int g = lane >> 2, t = lane & 3;
   const BLayer& lay = sh.lay[l];
-  const float* st = a.stats + (long long)(3 * l) * a.R * 2;
+  const int NB = (3 * d + 127) >> 7, KA = d >> 6;  // the QKV GEMM's n-blocks and k-atoms
   __half* kc = a.kcache + (long long)l * a.kv_layer_stride;
   __half* vc = a.vcache + (long long)l * a.kv_layer_stride;
   const int ntasks = H * a.R, e0 = 2 * lane;
@@ -637,11 +678,12 @@ __device__ __noinline__ void bs_self_attn_phase(const BStepArgs& a, BsShared& sh
       const uint32_t sv = (jj < pos) ? (uint32_t)__ldg(anc + jj) : 0u;
       slots[i >> 2] |= sv << (8 * (i & 3));
     }
+    const float2 ss = bs_row_sums(a, r);
+    if (h == 0 && lane == 0) __stcg(reinterpret_cast<float2*>(a.stats) + (long long)(3 * l) * a.R + r, ss);
     float mean, rstd;
-    bs_row_stats(st, r, d, mean, rstd);
-    const float2 rq = __ldcg(reinterpret_cast<const float2*>(a.qkv32 + bs_bidx(a.R, r, h * 64 + e0))),
-                 rk = __ldcg(reinterpret_cast<const float2*>(a.qkv32 + bs_bidx(a.R, r, d + h * 64 + e0))),
-                 rv = __ldcg(reinterpret_cast<const float2*>(a.qkv32 + bs_bidx(a.R, r, 2 * d + h * 64 + e0)));
+    bs_row_norm(ss, d, mean, rstd);
+    const float2 rq = bs_part_sum<float2>(a, NB, KA, r, h * 64 + e0), rk = bs_part_sum<float2>(a, NB, KA, r, d + h * 64 + e0),
+                 rv = bs_part_sum<float2>(a, NB, KA, r, 2 * d + h * 64 + e0);
     const float* ws = lay.wsum[0] + h * 64 + e0;
     const float* bs = lay.bias[0] + h * 64 + e0;
     const float2 wq = __ldg(reinterpret_cast<const float2*>(ws)), wk = __ldg(reinterpret_cast<const float2*>(ws + d)),
@@ -812,21 +854,24 @@ __device__ __noinline__ void bs_cross_attn_phase(const BStepArgs& a, BsShared& s
   const BLayer& lay = sh.lay[l];
   BS_TICK_DECL(tp0);
   if (lane == 0 && nt > 1) mbar_arrive(&sh.kvfree[1]);  // the multi-purpose region is free for K/V tiles now (one arrival per warp)
-  // ---- queries of every group this run touches, in one round trip (deferred LayerNorm + bias, fp16 rounding, then the exact 1/8) ----
+  // ---- queries of every group this run touches: split-K sums of the cross-q partials, deferred LayerNorm + bias, fp16 rounding,
+  // then the exact 1/8 ----
   const int g_first = t0 / S, n_groups = (t1 - 1) / S - g_first + 1;
+  const int NB = (d + 127) >> 7, KA = d >> 6;  // the cross-q GEMM's n-blocks and k-atoms
   for (int idx = tid; idx < n_groups * 64; idx += kBsThreads) {
     const int gi = idx >> 6, q = (idx & 63) >> 3, c = idx & 7;
     const int grp = g_first + gi, h = grp % a.H, b = grp / a.H;
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
     if (q < nq) {
       const int r = b * nq + q;
+      const float2 ss = bs_row_sums(a, r);
+      if (h == 0 && c == 0) __stcg(reinterpret_cast<float2*>(a.stats) + (long long)(3 * l + 1) * a.R + r, ss);
       float mean, rstd;
-      bs_row_stats(a.stats + (long long)(3 * l + 1) * a.R * 2, r, d, mean, rstd);
+      bs_row_norm(ss, d, mean, rstd);
       const float mr = mean * rstd;
-      const float* raw = a.cq32 + bs_bidx(a.R, r, h * 64 + c * 8);
       const float* ws = lay.wsum[1] + h * 64 + c * 8;
       const float* bs = lay.bias[2] + h * 64 + c * 8;
-      const float4 r0 = __ldcg(reinterpret_cast<const float4*>(raw)), r1 = __ldcg(reinterpret_cast<const float4*>(raw) + 1);
+      const float4 r0 = bs_part_sum<float4>(a, NB, KA, r, h * 64 + c * 8), r1 = bs_part_sum<float4>(a, NB, KA, r, h * 64 + c * 8 + 4);
       const float4 w0 = __ldg(reinterpret_cast<const float4*>(ws)), w1 = __ldg(reinterpret_cast<const float4*>(ws) + 1);
       const float4 b0 = __ldg(reinterpret_cast<const float4*>(bs)), b1 = __ldg(reinterpret_cast<const float4*>(bs) + 1);
 #define BS_FIX(raw_, w_, b_) fmaf(rstd, raw_, fmaf(-mr, w_, b_))
@@ -1055,48 +1100,6 @@ __device__ __noinline__ void bs_cross_attn_phase(const BStepArgs& a, BsShared& s
   }
 }
 
-// h16 = GELU(rstd (h32 - mean rowsum(W1)) + b1), evaluated once per element; h32 is zeroed for the next layer's sums.
-// A thread keeps ONE column group (4 channels: folded row sum and bias loaded once) and walks the rows with a stride, the next
-// row's loads in flight while the current one is evaluated: one index division per run, a rolled loop, ~200 instructions instead of
-// the 900 of an unrolled version (this runs once per layer: its cost is its instruction count).
-__device__ __noinline__ void bs_gelu_phase(const BStepArgs& a, BsShared& sh, int l) {
-  const int d = a.d, R = a.R, wr0 = 0, r_end = R;
-  const BLayer& lay = sh.lay[l];
-  const float2* st = reinterpret_cast<const float2*>(a.stats + (long long)(3 * l + 2) * R * 2);
-  const int gtid = blockIdx.x * kBsThreads + threadIdx.x, per_row = d;  // float4 units per row of 4d
-  const int rstride = (gridDim.x * kBsThreads) / per_row;               // rows one sweep of the grid covers (>= 1: grid >= 8 CTAs, d <= 1280)
-  const int rr = gtid / per_row, n = (gtid - rr * per_row) * 4;
-  if (rr < rstride) {
-    const float4 ws = __ldg(reinterpret_cast<const float4*>(lay.wsum[2] + n)), bb = __ldg(reinterpret_cast<const float4*>(lay.bias[4] + n));
-    int r = wr0 + rr;
-    float4 hv = make_float4(0.f, 0.f, 0.f, 0.f);
-    float2 sv = make_float2(0.f, 0.f);
-    if (r < r_end) {
-      hv = __ldcg(reinterpret_cast<const float4*>(a.h32 + bs_bidx(R, r, n)));
-      sv = __ldcg(st + r);
-    }
-#pragma unroll 1
-    while (r < r_end) {
-      const int rn = r + rstride;
-      float4 hn = hv;
-      float2 sn = sv;
-      if (rn < r_end) {  // the next row's loads fly while this one is evaluated
-        hn = __ldcg(reinterpret_cast<const float4*>(a.h32 + bs_bidx(R, rn, n)));
-        sn = __ldcg(st + rn);
-      }
-      const float mean = sv.x / d;
-      const float rstd = rsqrtf(fmaxf(sv.y / d - mean * mean, 0.f) + 1e-5f);
-      const float mr = mean * rstd;
-      const float y0 = gelu_erf(fmaf(rstd, hv.x, fmaf(-mr, ws.x, bb.x))), y1 = gelu_erf(fmaf(rstd, hv.y, fmaf(-mr, ws.y, bb.y)));
-      const float y2 = gelu_erf(fmaf(rstd, hv.z, fmaf(-mr, ws.z, bb.z))), y3 = gelu_erf(fmaf(rstd, hv.w, fmaf(-mr, ws.w, bb.w)));
-      *reinterpret_cast<uint2*>(a.h16 + (long long)r * 4 * d + n) = make_uint2(pack_half2(y0, y1), pack_half2(y2, y3));
-      hv = hn;
-      sv = sn;
-      r = rn;
-    }
-  }
-}
-
 // xn16[r] = (x[r] - mean) * rstd  (CTA r; the final LayerNorm's affine part is folded into the output embedding)
 __device__ __noinline__ void bs_final_ln_phase(const BStepArgs& a, float* red) {
   const int r = blockIdx.x, d = a.d, tid = threadIdx.x;
@@ -1253,7 +1256,7 @@ __global__ void __launch_bounds__(kBsLaunch, 1) bstep_kernel(const BStepArgs a_p
 #pragma unroll 1
     for (int l = 0; l < L && run; ++l) {
 #pragma unroll 1
-      for (int ph = 0; ph < 9 && run; ++ph) {
+      for (int ph = 0; ph < 8 && run; ++ph) {
         switch (ph) {
           case 0: bs_gemm_phase(a, sh, 6 * l + 0, U, ring); break;
           case 1: bs_self_attn_phase(a, sh, l, U); break;
@@ -1262,7 +1265,6 @@ __global__ void __launch_bounds__(kBsLaunch, 1) bstep_kernel(const BStepArgs a_p
           case 4: bs_cross_attn_phase(a, sh, l, kv0, U); break;
           case 5: bs_gemm_phase(a, sh, 6 * l + 3, U, ring); break;
           case 6: bs_gemm_phase(a, sh, 6 * l + 4, U, ring); break;
-          case 7: bs_gelu_phase(a, sh, l); break;
           default: bs_gemm_phase(a, sh, 6 * l + 5, U, ring); break;
         }
         run = bs_enabled(a, ++phase);
@@ -1371,7 +1373,7 @@ static int bstep_max_dynamic_smem() {
 
 void bstep_configure() { B2W_CUDA(cudaFuncSetAttribute(bstep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bstep_max_dynamic_smem())); }
 
-int bstep_phase_count(int L) { return 3 + 9 * L; }
+int bstep_phase_count(int L) { return 3 + 8 * L; }
 
 size_t bstep_xpart_floats(const BStepArgs& a) { return (size_t)a.n_chunks * a.H * kDsXSplits * kBsXQ * 66; }
 
@@ -1424,23 +1426,23 @@ void bstep_launch(const BStepArgs& a, int grid, cudaStream_t s) {
 // prof + 3000, written by bstep_kernel into a.prof; the counters are cleared after printing.
 void bstep_print_profile(const BStepArgs& a, cudaStream_t s) {
   B2W_CUDA(cudaStreamSynchronize(s));
-  const int L = a.L, nstamps = 1 + 2 * (2 + 9 * L) + 1;
+  const int L = a.L, nstamps = 1 + 2 * (2 + 8 * L) + 1;
   std::vector<unsigned long long> t(nstamps);
   B2W_CUDA(cudaMemcpy(t.data(), a.prof, nstamps * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  static const char* names[9] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1", "gelu", "ffn2"};
-  double work[9] = {0}, wait[9] = {0};
+  static const char* names[8] = {"qkv", "self_attn", "out_proj", "cross_q", "cross_attn", "cross_out", "ffn1+gelu", "ffn2"};
+  double work[8] = {0}, wait[8] = {0};
   unsigned long long prev = t[2];
   for (int l = 0; l < L; ++l)
-    for (int ph = 0; ph < 9; ++ph) {
-      const int bi = 1 + 2 * (1 + l * 9 + ph);
+    for (int ph = 0; ph < 8; ++ph) {
+      const int bi = 1 + 2 * (1 + l * 8 + ph);
       work[ph] += double(t[bi] - prev);
       wait[ph] += double(t[bi + 1] - t[bi]);
       prev = t[bi + 1];
     }
-  const int bf = 1 + 2 * (1 + 9 * L);
+  const int bf = 1 + 2 * (1 + 8 * L);
   fprintf(stderr, "[bstep prof] last step (R=%d): total %.1f us; embed %.1f us; final-LN %.1f us; logits %.1f us\n", a.R, (t[nstamps - 1] - t[0]) / 1e3,
           (t[2] - t[0]) / 1e3, (t[bf] - prev) / 1e3, (t[nstamps - 1] - t[bf + 1]) / 1e3);
-  for (int ph = 0; ph < 9; ++ph)
+  for (int ph = 0; ph < 8; ++ph)
     fprintf(stderr, "[bstep prof]   %-10s work %.2f us  barrier wait %.2f us (CTA 0, mean over %d layers)\n", names[ph], work[ph] / L / 1e3,
             wait[ph] / L / 1e3, L);
   {

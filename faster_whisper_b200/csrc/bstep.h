@@ -34,13 +34,10 @@ struct BStepArgs {
   const RowInfo* rows;
   const int* tokens_in;
   float* x;       // [R][d]   fp32 residual stream
-  float* qkv32;   // [R][3d]  raw W_qkv x (split-K sums, reduced in a fixed order)
-  float* cq32;    // [R][d]   raw cross-attention query
-  float* h32;     // [R][4d]  raw FFN hidden
   __half* ao;     // [R][d]   attention output
   __half* h16;    // [R][4d]  GELU(hidden)
   __half* xn16;   // [R][d]   final LayerNorm output
-  float* stats;   // [3L][R][2]  sum(x), sum(x^2) of the residual stream at each LayerNorm
+  float* stats;   // [3L][R][2]  sum(x), sum(x^2) of the residual stream at each LayerNorm (a record for b2w_debug_fetch)
   float* stpart;  // [d/64][R][2] per-k-atom partials of the statistics of the current GEMM phase
   float* gpart;   // [grid][R][128] each CTA's split-K partial tile of the current GEMM phase
   float* logits;  // [R][vpad]

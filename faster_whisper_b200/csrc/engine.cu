@@ -750,9 +750,6 @@ static void ensure_decoder_ws(Model* m, int chunks, int slots) {
     m->d_ao = model_alloc<__half>(m, (size_t)kMaxRows * dt);
     m->d_h = model_alloc<__half>(m, (size_t)kMaxRows * 4 * dt);
     m->d_logits = model_alloc<float>(m, (size_t)kMaxRows * m->vpad);
-    m->d_qkv32 = model_alloc<float>(m, (size_t)kMaxRows * ceil_div(3 * dt, 128) * 128);
-    m->d_cq32 = model_alloc<float>(m, (size_t)kMaxRows * dt128);
-    m->d_h32 = model_alloc<float>(m, (size_t)kMaxRows * ceil_div(4 * dt, 128) * 128);
     m->d_h16 = model_alloc<__half>(m, (size_t)kMaxRows * 4 * dt);
     m->d_xn16 = model_alloc<__half>(m, (size_t)kMaxRows * dt);
     m->d_stats = model_alloc<float>(m, (size_t)3 * L * kMaxRows * 2 + 4);
@@ -1184,7 +1181,7 @@ static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const in
     bs.logit_atoms = m->logit_atoms; bs.logit_bias = m->logit_b; bs.logit_scale = m->logit_scale;
     if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // read per call: tools/bstep_bisect.py steps it
     bs.rows = sb.rows; bs.tokens_in = sb.tokens_in;
-    bs.x = m->d_x; bs.qkv32 = m->d_qkv32; bs.cq32 = m->d_cq32; bs.h32 = m->d_h32; bs.ao = m->d_ao; bs.h16 = m->d_h16; bs.xn16 = m->d_xn16;
+    bs.x = m->d_x; bs.ao = m->d_ao; bs.h16 = m->d_h16; bs.xn16 = m->d_xn16;
     bs.stats = m->d_stats; bs.stpart = m->d_stpart; bs.gpart = m->d_gpart; bs.logits = m->d_logits;
     bs.kcache = m->kcache; bs.vcache = m->vcache; bs.kv_layer_stride = (long long)m->kv_elems;
     bs.anc = sb.anc; bs.anc_buf_stride = (long long)n * K * c.n_text_ctx;
@@ -2146,9 +2143,8 @@ int b2w_debug_fetch(b2w_model* h, int32_t which, float* out, int64_t n) {
     const __half* f16 = nullptr;
     switch (which) {
       case 0: f32 = m->d_x; break;
-      case 1: f32 = m->d_qkv32; break;
-      case 2: f32 = m->d_cq32; break;
-      case 3: f32 = m->d_h32; break;
+      case 1: f32 = m->d_gpart; break;
+      case 2: f32 = m->d_stpart; break;
       case 4: f16 = m->d_ao; break;
       case 5: f16 = m->d_h16; break;
       case 6: f16 = m->d_xn16; break;

@@ -134,7 +134,7 @@ struct Model {
   BLayer* d_blayers = nullptr;
   const void* logit_atoms = nullptr;
   const float* logit_scale = nullptr;
-  float *d_qkv32 = nullptr, *d_cq32 = nullptr, *d_h32 = nullptr, *d_stats = nullptr, *d_gpart = nullptr, *d_stpart = nullptr;
+  float *d_stats = nullptr, *d_gpart = nullptr, *d_stpart = nullptr;
   __half *d_h16 = nullptr, *d_xn16 = nullptr;
   std::optional<StepPath> forced_step;  // B2W_STEP=dstep|bstep|layers (tests and tools)
   DecBindings h_bind{};

@@ -263,9 +263,10 @@ int b2w_debug_logits(b2w_model* m, b2w_encoded* e, const int32_t* tokens, int32_
 int b2w_debug_step_logits(b2w_model* m, b2w_encoded* e, const int32_t* prompts, int32_t P, int32_t n, int32_t K,
                           int32_t n_steps, const int32_t* tokens, const int32_t* parents, float* logits_out);
 
-/* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 raw QKV
- * sums [R][3d], 2 raw cross-q sums [R][d], 3 raw FFN hidden sums [R][4d], 4 attention output [R][d], 5 GELU(hidden) [R][4d],
- * 6 final LayerNorm output [R][d], 7 LayerNorm statistics [3L][80][2], 8 logits [R][vpad]; n = number of floats to copy.
+/* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 the
+ * many-row step kernel's split-K partial tiles of its last GEMM phase [CTA][R][128], 2 the per-k-atom partials of its last row
+ * statistics [d/64][R][2], 4 attention output [R][d], 5 GELU(hidden) [R][4d], 6 final LayerNorm output [R][d], 7 LayerNorm
+ * statistics [3L][80][2], 8 logits [R][vpad]; n = number of floats to copy.
  * With B2W_BSTEP_STOP=<p> the many-row step kernel stops after p grid phases, so this bisects it phase by phase. */
 int b2w_debug_fetch(b2w_model* m, int32_t which, float* out, int64_t n);
 

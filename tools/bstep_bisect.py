@@ -3,7 +3,8 @@
 Runs ONE decode step (prompt [sot, notimestamps], so the step feeds position 1 after a one-token prefill) with
 B2W_STEP=bstep and B2W_BSTEP_STOP=p for p = 1 .. number of grid phases, fetches the decoder workspace after each
 stop (b2w_debug_fetch) and compares it with a NumPy restatement of the same step.  Prints the max abs error per
-phase so one run bisects a wrong kernel.  Test infrastructure (imports oracle/ only for the log-mel features).
+phase so one run bisects a wrong kernel.  The QKV and cross-q outputs exist only as the CTAs' split-K partial tiles and
+per-k-atom row statistics (their consumers sum them): those are summed here in the kernel's order.  Test infrastructure (imports oracle/ only for the log-mel features).
 
     python tools/bstep_bisect.py [--chunks 2] [--beam 5] [--d 128] [--layers 2]
 """
@@ -114,7 +115,11 @@ def main():
     refs = [reference_step(w64, enc_np[b], toks, d, H, L) for b in range(B)]
     R = B * K
     vpad = (dims.n_vocab + 15) // 16 * 16
-    nph = 3 + 9 * L
+    nph = 3 + 8 * L
+    import torch
+
+    G = torch.cuda.get_device_properties(0).multi_processor_count  # the step kernel's grid: one CTA per SM
+    KA = d // 64
     last = args.last or nph
 
     def rows(key):
@@ -126,47 +131,66 @@ def main():
         raw = eng.debug_fetch(which, nb * R * 128).reshape(nb, R, 128)
         return raw.transpose(1, 0, 2).reshape(R, nb * 128)[:, :n_cols]
 
-    def fixed(raw, stats_slot, lname, wname, bname, stats):
+    def split_k_sum(n_cols):
+        """GEMM output [R][n_cols] from the partial tiles [CTA][R][128]: n-block nb is summed over its CTAs g0 .. g0 + gn - 1 in
+        CTA order, fp32 (bs_group in csrc/bstep.cu)."""
+        NB = (n_cols + 127) // 128
+        parts = eng.debug_fetch(1, G * R * 128).reshape(G, R, 128)
+        base, extra = G // NB, G % NB
+        out = np.zeros((R, NB * 128), np.float32)
+        for nb in range(NB):
+            g0, gn = nb * base + min(nb, extra), min(base + 1 if nb < extra else base, KA)
+            t = parts[g0].copy()
+            for k in range(1, gn):
+                t = t + parts[g0 + k]
+            out[:, nb * 128 : nb * 128 + 128] = t
+        return out[:, :n_cols]
+
+    def row_stats():
+        """sum(x), sum(x^2) per row: the per-k-atom partials [KA][R][2] summed in k order, fp32."""
+        stp = eng.debug_fetch(2, KA * R * 2).reshape(KA, R, 2)
+        t = stp[0].copy()
+        for k in range(1, KA):
+            t = t + stp[k]
+        return t.astype(np.float64)
+
+    def fixed(raw, lname, wname, bname, s):
         p_ln_g, p_ln_b = w64[lname + ".weight"], w64[lname + ".bias"]
         Ws = w64[wname] if isinstance(wname, str) else np.concatenate([w64[x] for x in wname])
         bs = np.concatenate([w64[x] if x in w64 else np.zeros(d) for x in bname]) if not isinstance(bname, str) else w64[bname]
         Wf = (Ws * p_ln_g[None, :]).astype(np.float16).astype(np.float64)
         bf = bs + Ws @ p_ln_b
-        s = stats[stats_slot, :R]
         mean = s[:, 0] / d
         rstd = 1.0 / np.sqrt(np.maximum(s[:, 1] / d - mean * mean, 0) + 1e-5)
         return rstd[:, None] * (raw - mean[:, None] * Wf.sum(1)[None, :]) + bf[None, :]
 
-    names = ["qkv", "self", "out", "cross_q", "cross", "cross_out", "ffn1", "gelu", "ffn2"]
+    names = ["qkv", "self", "out", "cross_q", "cross", "cross_out", "ffn1+gelu", "ffn2"]
+    ref_key = [0, 1, 2, 3, 4, 5, 7, 8]  # reference_step's value after each grid phase of a layer
     worst = 0.0
     for p in range(args.first, last + 1):
         os.environ["B2W_BSTEP_STOP"] = str(p)
         eng.generate(enc, [toks] * B, beam_size=K, max_length=len(toks) + 1, return_scores=True)
-        st_raw = eng.debug_fetch(7, 3 * L * R * 2).reshape(3 * L, R, 2).astype(np.float64)
         if p == 1:
             got, want, label = fetch_blocked(0, d), rows("embed"), "embed x"
-        elif p <= 1 + 9 * L:
-            l, ph = divmod(p - 2, 9)
+        elif p <= 1 + 8 * L:
+            l, ph = divmod(p - 2, 8)
             blk = f"decoder.blocks.{l}"
             label = f"L{l} {names[ph]}"
-            want = rows((l, ph))
+            want = rows((l, ref_key[ph]))
             if ph == 0:
-                raw = fetch_blocked(1, 3 * d).astype(np.float64)
-                got = fixed(raw, 3 * l, blk + ".attn_ln", [blk + ".attn.query.weight", blk + ".attn.key.weight", blk + ".attn.value.weight"],
-                            [blk + ".attn.query.bias", blk + ".attn.key.bias", blk + ".attn.value.bias"], st_raw)
+                raw = split_k_sum(3 * d).astype(np.float64)
+                got = fixed(raw, blk + ".attn_ln", [blk + ".attn.query.weight", blk + ".attn.key.weight", blk + ".attn.value.weight"],
+                            [blk + ".attn.query.bias", blk + ".attn.key.bias", blk + ".attn.value.bias"], row_stats())
             elif ph in (1, 4):
                 got = eng.debug_fetch(4, R * d).reshape(R, d)
-            elif ph in (2, 5, 8):
+            elif ph in (2, 5, 7):
                 got = fetch_blocked(0, d)
             elif ph == 3:
-                raw = fetch_blocked(2, d).astype(np.float64)
-                got = fixed(raw, 3 * l + 1, blk + ".cross_attn_ln", blk + ".cross_attn.query.weight", blk + ".cross_attn.query.bias", st_raw)
-            elif ph == 6:
-                raw = fetch_blocked(3, 4 * d).astype(np.float64)
-                got = fixed(raw, 3 * l + 2, blk + ".mlp_ln", blk + ".mlp.0.weight", blk + ".mlp.0.bias", st_raw)
+                raw = split_k_sum(d).astype(np.float64)
+                got = fixed(raw, blk + ".cross_attn_ln", blk + ".cross_attn.query.weight", blk + ".cross_attn.query.bias", row_stats())
             else:
                 got = eng.debug_fetch(5, R * 4 * d).reshape(R, 4 * d)
-        elif p == 2 + 9 * L:
+        elif p == 2 + 8 * L:
             got, want, label = eng.debug_fetch(6, R * d).reshape(R, d), rows("xn"), "final LN"
         else:
             got, want, label = eng.debug_fetch(8, R * vpad).reshape(R, vpad)[:, : dims.n_vocab], rows("logits"), "logits"
