@@ -1379,7 +1379,7 @@ size_t bstep_xpart_floats(const BStepArgs& a) { return (size_t)a.n_chunks * a.H 
 
 bool bstep_supported(int num_sms, BStepArgs& a) {
   if (a.R < 1 || a.R > kBsMaxRows || a.d % 64 != 0 || a.d > 1280 || a.d != 64 * a.H || a.L > 32 || a.rows_per_chunk > kBsXQ || num_sms < 8) return false;
-  if ((a.T + kDsXSplits - 1) / kDsXSplits + 1 > kDsXKeysMax || a.vpad % 4 != 0 || a.n_ctx > 448) return false;
+  if (a.vpad % 4 != 0 || a.n_ctx > 448) return false;
   {  // a CTA's run of cross-attention tiles may touch at most kBsXGroups (chunk, head) groups
     const int NT = kDsXSplits * a.H * a.n_chunks, run = (NT + num_sms - 1) / num_sms;
     if ((run + kDsXSplits - 1) / kDsXSplits + 1 > kBsXGroups) return false;

@@ -8,9 +8,7 @@
 //    *next* LayerNorm executed by the last CTA to finish (saves a launch per sub-layer), fp32 logits.
 //  * dec_self_attn : masked attention over the paged self-KV cache through the beam ancestry table
 //    (no gather-copy of the cache when beams reorder).
-//  * dec_cross_attn: beam-shared cross attention — each K/V tile of a chunk is read once for all of the
-//    chunk's beams (5x fewer bytes than CTranslate2's per-row replication), split over keys
-//    (flash-decoding) so B=1 still fills the GPU.
+// Cross attention is the persistent step's task launched on its own (dstep.cu, dstep_cross_attn_launch).
 //
 // Together these replace the per-token body of CTranslate2's Whisper.generate loop
 // (reference call sites faster_whisper/transcribe.py:222-236, 1446-1459; SURVEY.md §2.3 rows K10-K15).
@@ -345,198 +343,6 @@ __global__ void __launch_bounds__(128) dec_self_attn_kernel(const SelfAttnArgs a
 
 void dec_self_attn(const SelfAttnArgs& a, int R, int H, cudaStream_t s) {
   dec_self_attn_kernel<<<dim3(H, R), 128, 0, s>>>(a);
-  B2W_LAUNCHED();
-}
-
-// ---- beam-shared cross attention (split over keys) ---------------------------------------------------------------------
-constexpr int kXQ = 8;        // queries (rows of one chunk) per CTA
-constexpr int kXThreads = 128;
-
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
-}
-
-__global__ void __launch_bounds__(kXThreads) dec_cross_attn_kernel(const CrossAttnArgs a) {
-  extern __shared__ __align__(16) float sm[];
-  const int T = a.T, S = a.splits;
-  const int split = blockIdx.x % S, qg = blockIdx.x / S, h = blockIdx.y, b = blockIdx.z;
-  const int row0 = b * a.rows_per_chunk + qg * kXQ;
-  const int nq = min(kXQ, a.rows_per_chunk - qg * kXQ);
-  if (nq <= 0) return;
-  const int k0 = (int)((long long)T * split / S), k1 = (int)((long long)T * (split + 1) / S);
-  const int nk = k1 - k0;
-  const int kmax = (T + S - 1) / S + 1;
-  float* qs = sm;                     // [kXQ][64]
-  float* sc = qs + kXQ * 64;          // [kXQ][kmax]
-  float* wred = sc + kXQ * kmax;      // [4][kXQ][64]
-  float* stat = wred + 4 * kXQ * 64;  // [kXQ][2]
-  __half* vt = reinterpret_cast<__half*>(stat + kXQ * 2);  // [kmax][64] V tile; float offset 512 + 8*kmax + 2048 + 16 is a multiple of 4 -> 16-byte aligned
-  __half* kt = vt + kmax * 64;                             // [kmax][72] K tile, rows padded to 144 B: conflict-free 16-byte reads by one thread per key
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int d = a.d;
-  const DecBindings bd = *a.bind;
-  const long long per = (long long)bd.B_total * a.H * T * 64;  // one layer's K (or V) block
-  const __half* Kb = bd.xkv + ((long long)a.layer * 2 + 0) * per + (((long long)(bd.chunk0 + b) * a.H + h) * T) * 64;
-  const __half* Vb = bd.xkv + ((long long)a.layer * 2 + 1) * per + (((long long)(bd.chunk0 + b) * a.H + h) * T) * 64;
-  // K and V tiles -> shared memory with fully coalesced 16-byte async copies (every byte of the beam-shared
-  // cross-KV cache crosses HBM once per chunk and step); V's latency hides behind the score phase
-  // (the cache stores each 128-byte row with its 16-byte chunks at chunk ^ (t & 7), gemm.cu EPI_F16_XKV: undo it here)
-  for (int i = tid; i < nk * 8; i += kXThreads) {
-    const int key = k0 + (i >> 3);
-    cp_async16(kt + (i >> 3) * 72 + (i & 7) * 8, Kb + (long long)key * 64 + (((i & 7) ^ (key & 7)) << 3));
-  }
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  for (int i = tid; i < nk * 8; i += kXThreads) {
-    const int key = k0 + (i >> 3);
-    cp_async16(vt + i * 8, Vb + (long long)key * 64 + (((i & 7) ^ (key & 7)) << 3));
-  }
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  for (int i = tid; i < kXQ * 64; i += kXThreads) {
-    const int q = i >> 6, e = i & 63;
-    qs[i] = (q < nq) ? __half2float(a.q[(long long)(row0 + q) * d + h * 64 + e]) * 0.125f : 0.f;
-  }
-  asm volatile("cp.async.wait_group 1;" ::: "memory");
-  __syncthreads();
-  // phase 1: scores, one key per thread
-  for (int j = tid; j < nk; j += kXThreads) {
-    const uint4* kp = reinterpret_cast<const uint4*>(kt + j * 72);
-    float kf[64];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const uint4 kr = kp[i];
-      const __half2* k2 = reinterpret_cast<const __half2*>(&kr);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __half22float2(k2[e]);
-        kf[8 * i + 2 * e] = f.x;
-        kf[8 * i + 2 * e + 1] = f.y;
-      }
-    }
-    for (int q = 0; q < nq; ++q) {
-      const float4* q4 = reinterpret_cast<const float4*>(qs + q * 64);
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float4 qq = q4[i];
-        s = fmaf(qq.x, kf[4 * i], s);
-        s = fmaf(qq.y, kf[4 * i + 1], s);
-        s = fmaf(qq.z, kf[4 * i + 2], s);
-        s = fmaf(qq.w, kf[4 * i + 3], s);
-      }
-      sc[q * kmax + j] = s;
-    }
-  }
-  __syncthreads();
-  // phase 2: per-query partial softmax statistics (warp per query)
-  for (int q = warp; q < kXQ; q += 4) {
-    if (q < nq) {
-      float mx = -INFINITY;
-      for (int j = lane; j < nk; j += 32) mx = fmaxf(mx, sc[q * kmax + j]);
-      mx = warp_max(mx);
-      float sum = 0.f;
-      for (int j = lane; j < nk; j += 32) {
-        const float p = __expf(sc[q * kmax + j] - mx);
-        sc[q * kmax + j] = p;
-        sum += p;
-      }
-      sum = warp_sum(sum);
-      if (lane == 0) {
-        stat[q * 2] = mx;
-        stat[q * 2 + 1] = sum;
-      }
-    } else {
-      for (int j = lane; j < nk; j += 32) sc[q * kmax + j] = 0.f;  // unused query slots contribute nothing
-    }
-  }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-  __syncthreads();
-  // phase 3: P*V from shared memory, lane owns 2 dims, warps split keys
-  float acc[kXQ][2];
-#pragma unroll
-  for (int q = 0; q < kXQ; ++q) acc[q][0] = acc[q][1] = 0.f;
-  for (int j = warp; j < nk; j += 4) {
-    const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(vt + j * 64 + 2 * lane));
-#pragma unroll
-    for (int q = 0; q < kXQ; ++q) {
-      const float p = sc[q * kmax + j];
-      acc[q][0] = fmaf(p, vf.x, acc[q][0]);
-      acc[q][1] = fmaf(p, vf.y, acc[q][1]);
-    }
-  }
-#pragma unroll
-  for (int q = 0; q < kXQ; ++q) {
-    wred[(warp * kXQ + q) * 64 + 2 * lane] = acc[q][0];
-    wred[(warp * kXQ + q) * 64 + 2 * lane + 1] = acc[q][1];
-  }
-  __syncthreads();
-  // partials: part[(b,h,qg)][split][q][66]: 64 acc + m + l
-  const long long group = ((long long)b * a.H + h) * a.qgroups + qg;
-  float* part = a.partial + (group * S + split) * (kXQ * 66);
-  for (int i = tid; i < nq * 64; i += kXThreads) {
-    const int q = i >> 6, e = i & 63;
-    part[q * 66 + e] = wred[(0 * kXQ + q) * 64 + e] + wred[(1 * kXQ + q) * 64 + e] + wred[(2 * kXQ + q) * 64 + e] + wred[(3 * kXQ + q) * 64 + e];
-  }
-  if (tid < nq) {
-    part[tid * 66 + 64] = stat[tid * 2];
-    part[tid * 66 + 65] = stat[tid * 2 + 1];
-  }
-  __shared__ int is_last;
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    const int ticket = atomicAdd(a.counters + group, 1);
-    is_last = (ticket == S - 1);
-    if (is_last) a.counters[group] = 0;
-  }
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  // combine the S partials (S <= 8): all L2 loads are issued before they are consumed
-  const float* pg = a.partial + group * S * (kXQ * 66);
-  for (int i = tid; i < nq * 64; i += kXThreads) {
-    const int q = i >> 6, e = i & 63;
-    float pm[8], pl[8], pa[8];
-#pragma unroll
-    for (int s2 = 0; s2 < 8; ++s2) {
-      const bool on = s2 < S;
-      const float* base = pg + ((on ? s2 : 0) * kXQ + q) * 66;
-      pm[s2] = on ? __ldcg(base + 64) : -INFINITY;
-      pl[s2] = on ? __ldcg(base + 65) : 0.f;
-      pa[s2] = on ? __ldcg(base + e) : 0.f;
-    }
-    float M = pm[0];
-#pragma unroll
-    for (int s2 = 1; s2 < 8; ++s2) M = fmaxf(M, pm[s2]);
-    float num = 0.f, den = 0.f;
-#pragma unroll
-    for (int s2 = 0; s2 < 8; ++s2) {
-      const float w = (s2 < S) ? __expf(pm[s2] - M) : 0.f;
-      num = fmaf(w, pa[s2], num);
-      den = fmaf(w, pl[s2], den);
-    }
-    a.out[(long long)(row0 + q) * d + h * 64 + e] = __float2half_rn(num / den);
-  }
-}
-
-int cross_attn_smem_bytes(int T, int splits) {
-  const int kmax = (T + splits - 1) / splits + 1;
-  const int floats = kXQ * 64 + kXQ * kmax + 4 * kXQ * 64 + kXQ * 2;
-  return floats * (int)sizeof(float) + kmax * (64 + 72) * (int)sizeof(__half);
-}
-int cross_attn_qgroups(int rows_per_chunk) { return ceil_div(rows_per_chunk, kXQ); }
-size_t cross_attn_partial_floats(int B, int H, int rows_per_chunk, int splits) {
-  return (size_t)B * H * cross_attn_qgroups(rows_per_chunk) * splits * kXQ * 66;
-}
-
-void decode_configure() {
-  B2W_CUDA(cudaFuncSetAttribute(dec_cross_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-}
-
-void dec_cross_attn(const CrossAttnArgs& a, int B, cudaStream_t s) {
-  const int smem = cross_attn_smem_bytes(a.T, a.splits);
-  B2W_CHECK(smem <= 100 * 1024, "cross-attention tile too large");
-  dim3 grid(a.splits * a.qgroups, a.H, B);
-  dec_cross_attn_kernel<<<grid, kXThreads, smem, s>>>(a);
   B2W_LAUNCHED();
 }
 

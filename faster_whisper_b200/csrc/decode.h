@@ -60,21 +60,7 @@ struct DecBindings {
   int chunk0;
 };
 
-struct CrossAttnArgs {
-  const __half* q;   // [R][d], rows of a chunk contiguous
-  const DecBindings* bind;
-  int layer;
-  __half* out;       // [R][d]
-  float* partial;
-  int* counters;
-  int T, H, d, rows_per_chunk, splits, qgroups;
-};
-int cross_attn_smem_bytes(int T, int splits);
-int cross_attn_qgroups(int rows_per_chunk);
-size_t cross_attn_partial_floats(int B, int H, int rows_per_chunk, int splits);
-void dec_cross_attn(const CrossAttnArgs& a, int B, cudaStream_t s);
-void decode_configure();  // per-device kernel attributes (must run outside stream capture)
-void search_configure();
+void search_configure();  // per-device kernel attributes (must run outside stream capture)
 
 // ---- search (search.cu) ------------------------------------------------------------------------------------
 constexpr int kMaxBeam = 16;       // rows per chunk (beam_size or best_of)

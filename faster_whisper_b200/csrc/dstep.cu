@@ -41,7 +41,6 @@ namespace b2w {
 constexpr int kDsThreads = 256;   // compute threads (8 warps)
 constexpr int kDsLaunchThreads = 320;  // + one warp streaming weight tiles, one prefetching cross-attention K/V
 constexpr int kDsWarps = 8;
-constexpr int kDsXQ = 8;
 constexpr int kDsNBuf = 3;         // weight-tile ring: the tile being consumed + two in flight
 constexpr int kDsSelfKeys = 192;   // keys staged per self-attention pass
 constexpr int kDsKvBytes = 2 * kDsXKeysMax * 64 * 2;  // cross-attention K + V tile
@@ -415,10 +414,14 @@ __device__ __noinline__ void ds_self_attn_task(const DStepArgs& a, const DsShare
   ds_sync();
 }
 
-// TMA the K and V tiles of one cross-attention task (key split of one (chunk, head)) into kvbuf (one thread).
+// Cross-attention tasks: task = ((chunk * H + head) * QG + query group) * kDsXSplits + key split, with QG = ds_xqgroups(rows
+// per chunk); task / kDsXSplits indexes the task's partials and counter.
+__host__ __device__ __forceinline__ int ds_xtasks(const DStepArgs& a) { return kDsXSplits * ds_xqgroups(a.rows_per_chunk) * a.H * a.n_chunks; }
+
+// TMA the K and V tiles of one cross-attention task into kvbuf (one thread); they depend on (key split, head, chunk) only.
 __device__ __noinline__ void ds_issue_cross_kv(const DStepArgs& a, DsShared& sh, int layer, int task, unsigned char* kvbuf) {
-  const int split = task % kDsXSplits, rest = task / kDsXSplits;
-  const int h = rest % a.H, b = rest / a.H, T = a.T;
+  const int split = task % kDsXSplits, bh = task / kDsXSplits / ds_xqgroups(a.rows_per_chunk);
+  const int h = bh % a.H, b = bh / a.H, T = a.T;
   const int k0 = (int)((long long)T * split / kDsXSplits), k1 = (int)((long long)T * (split + 1) / kDsXSplits), nk = k1 - k0;
   const DecBindings bd = *a.bind;
   const long long per = (long long)bd.B_total * a.H * T * 64;
@@ -434,7 +437,7 @@ __device__ __noinline__ void ds_issue_cross_kv(const DStepArgs& a, DsShared& sh,
 // K/V producer (one thread of a second dedicated warp): per layer, as soon as the layer's self-attention has released the
 // buffer, fetch the tile of this CTA's first cross-attention task — it does not depend on the step, only on the layer.
 __device__ __noinline__ void ds_kv_producer(const DStepArgs& a, DsShared& sh, unsigned char* kvbuf) {
-  if ((int)blockIdx.x >= kDsXSplits * a.H * a.n_chunks) return;
+  if ((int)blockIdx.x >= ds_xtasks(a)) return;
 #pragma unroll 1
   for (int l = 0; l < a.L; ++l) {
     mbar_wait(&sh.kvfree, (uint32_t)(l & 1));
@@ -442,17 +445,18 @@ __device__ __noinline__ void ds_kv_producer(const DStepArgs& a, DsShared& sh, un
   }
 }
 
-// Beam-shared cross attention: one (key split, head, chunk) task for all rows of the chunk; the last split of a
-// (chunk, head) group to finish combines.  K/V rows are 128 bytes whose 16-byte chunks are XOR-swizzled by (key & 7) in the
-// cache itself (gemm.cu EPI_F16_XKV), so the tile arrives conflict-free with two bulk copies.
+// Beam-shared cross attention: one (key split, query group, head, chunk) task for up to kDsXQ rows of the chunk; the last
+// split of a (chunk, head, query group) to finish combines.  K/V rows are 128 bytes whose 16-byte chunks are XOR-swizzled by
+// (key & 7) in the cache itself (gemm.cu EPI_F16_XKV), so the tile arrives conflict-free with two bulk copies.
 //   S[key][q]  = K Q^T      : mma A = K rows (keys), B = Q rows; 16-byte fragment loads, k-permuted like the GEMVs
 //   O^T[e][q]  = V^T P^T    : mma A = V^T via ldmatrix.trans, B = P rows (fp16 probabilities)
 __device__ __noinline__ int ds_cross_attn_task(const DStepArgs& a, DsShared& sh, int layer, int task, bool prefetched, int kv_uses,
                                                unsigned char* kvbuf, unsigned char* scratch) {
   const int T = a.T, S = kDsXSplits, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int split = task % S, rest = task / S, h = rest % a.H, b = rest / a.H;
-  const int nq = a.rows_per_chunk, row0 = b * a.rows_per_chunk, d = a.d;
+  const int split = task % S, group = task / S, QG = ds_xqgroups(a.rows_per_chunk), qg = group % QG;
+  const int h = group / QG % a.H, b = group / QG / a.H, d = a.d;
+  const int row0 = b * a.rows_per_chunk + kDsXQ * qg, nq = min(kDsXQ, a.rows_per_chunk - kDsXQ * qg);
   const int k0 = (int)((long long)T * split / S), k1 = (int)((long long)T * (split + 1) / S), nk = k1 - k0;
   const int nkp = (nk + 15) & ~15;
   __half* kt = reinterpret_cast<__half*>(kvbuf);  // [224][64] swizzled
@@ -543,8 +547,7 @@ __device__ __noinline__ int ds_cross_attn_task(const DStepArgs& a, DsShared& sh,
     w[(2 * t + 1) * 64 + 16 * dtile + g + 8] = acc[3];
   }
   ds_sync();
-  const long long group = (long long)b * a.H + h;
-  float* part = a.xpart + (group * S + split) * (kDsXQ * 66);
+  float* part = a.xpart + ((long long)group * S + split) * (kDsXQ * 66);
 #pragma unroll 1
   for (int i = tid; i < nq * 64; i += kDsThreads) {
     const int q = i >> 6, e = i & 63;
@@ -563,7 +566,7 @@ __device__ __noinline__ int ds_cross_attn_task(const DStepArgs& a, DsShared& sh,
   }
   ds_sync();
   if (sh.flag) {
-    const float* pg = a.xpart + group * S * (kDsXQ * 66);
+    const float* pg = a.xpart + (long long)group * S * (kDsXQ * 66);
 #pragma unroll 1
     for (int i = tid; i < nq * 64; i += kDsThreads) {
       const int q = i >> 6, e = i & 63;
@@ -653,7 +656,7 @@ __global__ void __launch_bounds__(kDsLaunchThreads, 1) dstep_kernel(const DStepA
   }
   ds_grid_barrier(a, sh);
 
-  const int xtasks = kDsXSplits * a.H * a.n_chunks;
+  const int xtasks = ds_xtasks(a);
 #pragma unroll 1
   for (int l = 0; l < L; ++l) {
     __half* kc = a.kcache + (long long)l * a.kv_layer_stride;
@@ -691,7 +694,7 @@ __global__ void __launch_bounds__(kDsLaunchThreads, 1) dstep_kernel(const DStepA
 }
 
 // The same cross-attention task as a stand-alone kernel for the multi-kernel step (many chunks per call): one CTA per
-// (key split, head, chunk), ~74 KB of shared memory so three CTAs per SM overlap each other's tile fetches.
+// task, ~74 KB of shared memory so three CTAs per SM overlap each other's tile fetches.
 __global__ void __launch_bounds__(kDsThreads) ds_cross_attn_kernel(const DStepArgs a_param, int layer) {
   extern __shared__ __align__(128) unsigned char ds_smem[];
   __shared__ DStepArgs a_sh;
@@ -705,14 +708,10 @@ __global__ void __launch_bounds__(kDsThreads) ds_cross_attn_kernel(const DStepAr
   ds_cross_attn_task(a_sh, sh, layer, blockIdx.x, false, 0, ds_smem, ds_smem + kDsKvBytes);
 }
 
-bool dstep_cross_attn_supported(int T, int rows_per_chunk) {
-  return rows_per_chunk <= kDsXQ && (T + kDsXSplits - 1) / kDsXSplits + 1 <= kDsXKeysMax;
-}
-
 // a: q, ao, bind, xpart, xcounters, H, T, d, rows_per_chunk, n_chunks
 void dstep_cross_attn_launch(const DStepArgs& a, int layer, cudaStream_t s) {
   const size_t smem = kDsKvBytes + ((kDsXScratch + 127) & ~127);
-  ds_cross_attn_kernel<<<kDsXSplits * a.H * a.n_chunks, kDsThreads, smem, s>>>(a, layer);
+  ds_cross_attn_kernel<<<ds_xtasks(a), kDsThreads, smem, s>>>(a, layer);
   B2W_LAUNCHED();
 }
 
@@ -808,7 +807,7 @@ int dstep_max_grid(int num_sms, const DStepArgs& a) {
   const size_t smem = dstep_smem_bytes(a);
   const size_t self_scratch = (size_t)(kDsSelfKeys + 16 + 256 + 64) * sizeof(float) + (size_t)kDsSelfKeys * (72 + 64) * sizeof(__half);
   if (smem > 220 * 1024 || self_scratch > (size_t)kDsKvBytes) return 0;
-  if (a.d % 64 != 0 || a.d > 1280 || a.L > 32 || a.R > 8 || (a.T + kDsXSplits - 1) / kDsXSplits + 1 > kDsXKeysMax || num_sms < 4) return 0;
+  if (a.d % 64 != 0 || a.d > 1280 || a.L > 32 || a.R > 8 || num_sms < 4) return 0;
   int per_sm = 0;
   if (a.w8)
     B2W_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dstep_kernel<true>, kDsLaunchThreads, smem));

@@ -6,6 +6,9 @@ namespace b2w {
 
 constexpr int kDsXSplits = 7;    // key splits of the beam-shared cross attention (20 heads x 7 = 140 tasks, about one per SM)
 constexpr int kDsXKeysMax = 224;  // keys per cross-attention tile (multiple of 16, >= ceil(T / kDsXSplits) + 1)
+static_assert((B2W_N_AUDIO_CTX + kDsXSplits - 1) / kDsXSplits + 1 <= kDsXKeysMax, "a key split of the encoder output must fit one tile");
+constexpr int kDsXQ = 8;  // query rows per cross-attention task: a chunk's rows form ceil(rows_per_chunk / 8) query groups
+__host__ __device__ __forceinline__ int ds_xqgroups(int rows_per_chunk) { return (rows_per_chunk + kDsXQ - 1) / kDsXQ; }
 
 // Per layer: the six weight matrices of the step re-laid out as a stream of work-item tiles (dstep_pack_tiles), in the order
 // qkv, out, cross_q, cross_out, ffn1, ffn2.
@@ -53,8 +56,7 @@ void dstep_quantize_rows(__half* W, int N, int K, unsigned char* q, float* scale
 void dstep_pack_tiles_i8(const unsigned char* q, const float* scale, const float* bias, int N, int K, int ksplit, unsigned char* out,
                          cudaStream_t s);
 
-// stand-alone beam-shared cross attention on mma.sync (the persistent kernel's task as its own launch)
-bool dstep_cross_attn_supported(int T, int rows_per_chunk);
+// stand-alone beam-shared cross attention on mma.sync (the persistent kernel's task as its own launch), any rows per chunk
 void dstep_cross_attn_launch(const DStepArgs& a, int layer, cudaStream_t s);
 
 size_t dstep_smem_bytes(const DStepArgs& a);

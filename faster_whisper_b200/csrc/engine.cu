@@ -474,7 +474,6 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
   B2W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->h_pinned), 4096));
   m->d_suppress = model_alloc<uint8_t>(m, m->vpad);
   m->d_bind = model_alloc<DecBindings>(m, 1);
-  decode_configure();
   search_configure();
   gemm_configure();
   dstep_configure();
@@ -932,15 +931,10 @@ static void bind_encoded(Model* m, const Encoded* e, int chunk0) {
   B2W_CUDA(cudaMemcpyAsync(m->d_bind, &m->h_bind, sizeof(DecBindings), cudaMemcpyHostToDevice, m->stream));
 }
 
-// 8 key splits (~188 keys each) for the SIMT cross attention: the V tile fits in shared memory next to the scores and even one
-// chunk fills the SMs
-constexpr int kXSplits = 8;
-static_assert(kXSplits >= kDsXSplits, "the SIMT kernel's partial buffer must also hold the mma.sync task's partials");
-
-// Floats of the cross-attention partial buffer for n_chunks x rows_per_chunk rows.  The SIMT kernel's need (kXSplits splits per
-// query group) covers the kDsXSplits-split mma.sync task of both persistent kernels and of its stand-alone launch.
+// Floats of the cross-attention partial buffer for n_chunks x rows_per_chunk rows: 64 outputs + max + sum per (chunk, head,
+// query group, key split) and query row.
 static size_t xpart_floats(const Model* m, int n_chunks, int rows_per_chunk) {
-  return cross_attn_partial_floats(n_chunks, m->cfg.n_text_head, rows_per_chunk, kXSplits);
+  return (size_t)n_chunks * m->cfg.n_text_head * ds_xqgroups(rows_per_chunk) * kDsXSplits * kDsXQ * 66;
 }
 
 // The partial buffer is grown outside graph capture (which forbids cudaMalloc and synchronisation), before any argument block
@@ -970,9 +964,8 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
   cudaStream_t s = m->stream;
   const SearchBuffers& sb = m->sb;
   embed_ln(sb.tokens_in, sb.rows, m->tok_emb, m->dec_pos, nullptr, nullptr, m->d_x, m->d_xn, R, dt, c.n_vocab, s);
-  const int qgroups = cross_attn_qgroups(rows_per_chunk);
   B2W_CHECK(m->d_xpart_floats >= xpart_floats(m, n_chunks, rows_per_chunk), "cross-attention partial buffer");
-  B2W_CHECK((size_t)n_chunks * H * qgroups <= 16 * 20 * 64, "cross-attention group counters");
+  B2W_CHECK((size_t)n_chunks * H * ds_xqgroups(rows_per_chunk) <= 16 * 20 * 64, "cross-attention group counters");
   for (int l = 0; l < L; ++l) {
     const DecLayerW& W = m->dec[l];
     __half* kc = m->kcache + (size_t)l * m->kv_elems;
@@ -991,20 +984,10 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     q.x = m->d_xn; q.W = W.wq_x; q.bias = W.bq_x; q.R = R; q.N = dt; q.K = dt; q.mode = GV_F16; q.out_h = m->d_q;
     gv(m, q);
     if (cap) align_probs(m->d_q, m->d_bind, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, cap->pos0, R, H, 1500, dt, s);
-    if (dstep_cross_attn_supported(1500, rows_per_chunk)) {
-      DStepArgs xa{};
-      xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
-      xa.H = H; xa.T = 1500; xa.d = dt; xa.rows_per_chunk = rows_per_chunk; xa.n_chunks = n_chunks;
-      dstep_cross_attn_launch(xa, l, s);
-    } else {  // more than 8 rows per chunk: prefill passes, beams above 8
-      CrossAttnArgs ca;
-      ca.q = m->d_q;
-      ca.bind = m->d_bind;
-      ca.layer = l;
-      ca.out = m->d_ao; ca.partial = m->d_xpart; ca.counters = m->d_counters + 64;
-      ca.T = 1500; ca.H = H; ca.d = dt; ca.rows_per_chunk = rows_per_chunk; ca.splits = kXSplits; ca.qgroups = qgroups;
-      dec_cross_attn(ca, n_chunks, s);
-    }
+    DStepArgs xa{};
+    xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
+    xa.H = H; xa.T = 1500; xa.d = dt; xa.rows_per_chunk = rows_per_chunk; xa.n_chunks = n_chunks;
+    dstep_cross_attn_launch(xa, l, s);
     GvArgs ox;
     ox.x = m->d_ao; ox.W = W.wo_x; ox.bias = W.bo_x; ox.R = R; ox.N = dt; ox.K = dt; ox.mode = GV_RESID_LN;
     ox.xres = m->d_x; ox.xn_out = m->d_xn; ox.counter = m->d_counters;

@@ -179,7 +179,7 @@ def compare_with_oracle(runs, name, path, n, K, n_steps=STEPS, ct="default", **k
 
 DSTEP_SHAPES = [(1, 1), (1, 5), (1, 8), (2, 4), (8, 1), (3, 2)]
 BSTEP_SHAPES = [(1, 1), (1, 5), (2, 5), (4, 4), (17, 1), (4, 8), (11, 3), (16, 4), (13, 5), (16, 5), (10, 8)]
-LAYERS_SHAPES = [(16, 1), (17, 1), (6, 3), (5, 16), (16, 5)]
+LAYERS_SHAPES = [(16, 1), (17, 1), (6, 3), (5, 16), (16, 5), (1, 9)]
 CASES = [("dstep",) + s for s in DSTEP_SHAPES] + [("bstep",) + s for s in BSTEP_SHAPES] + [("layers",) + s for s in LAYERS_SHAPES]
 
 
@@ -188,7 +188,8 @@ CASES = [("dstep",) + s for s in DSTEP_SHAPES] + [("bstep",) + s for s in BSTEP_
 @pytest.mark.parametrize("path,n,K", CASES)
 def test_step_logits_match_oracle(runs, name, path, n, K):
     """Rows 1-8 through dstep (K = 8 cross-attention queries), bstep's padded row counts on both sides of 16, 32, 64 and at 80
-    with 1-8 rows per chunk, the layered step on both sides of its wgmma switch (17 rows) and with 16 rows per chunk."""
+    with 1-8 rows per chunk, the layered step on both sides of its wgmma switch (17 rows) and with 9 and 16 rows per chunk (a second
+    cross-attention query group of one row, two full groups)."""
     compare_with_oracle(runs, name, path, n, K)
 
 
