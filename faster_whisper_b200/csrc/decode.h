@@ -65,7 +65,10 @@ void search_configure();  // per-device kernel attributes (must run outside stre
 // ---- search (search.cu) ------------------------------------------------------------------------------------
 constexpr int kMaxBeam = 16;       // rows per chunk (beam_size or best_of)
 constexpr int kMaxCand = 2 * kMaxBeam;
-constexpr int kMaxFinished = 32;   // >= round(beam*patience) finished hypotheses kept per chunk
+constexpr int kMaxFinishTarget = 32;  // largest round(beam * patience): a chunk stops once it has this many finished hypotheses
+// Finished hypotheses kept per chunk.  Up to K hypotheses finish in one step, so a chunk that stops at max_finished can end with
+// max_finished + K - 1 of them; every one is kept, as CTranslate2 does (32 + 16 - 1, rounded up).
+constexpr int kMaxFinished = 48;
 
 struct SearchParams {
   int n_vocab, vpad;           // real vocabulary and padded logits row stride
@@ -74,7 +77,7 @@ struct SearchParams {
   int ncand;                   // beam: 2K ; greedy: 1
   int max_steps;               // generated tokens allowed (max_length - prompt_len)
   int prompt_len;
-  int max_finished;            // round(K * patience)
+  int max_finished;            // round(K * patience), at most kMaxFinishTarget
   int allow_early_exit;
   int num_hyp;
   float length_penalty, repetition_penalty;

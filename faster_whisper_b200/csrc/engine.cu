@@ -1040,8 +1040,7 @@ static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const i
 
 // ---- generate: one group of n chunks x K rows --------------------------------------------------------------------------------
 // Position of <|startoftranscript|>, which must be the same in every prompt of the group.
-static int validate_prompts(const Model* m, const int32_t* prompts, int n, int P) {
-  const b2w_config& c = m->cfg;
+static int validate_prompts(const b2w_config& c, const int32_t* prompts, int n, int P) {
   int sot_index = -1;
   for (int b = 0; b < n; ++b) {
     const int32_t* p = prompts + (size_t)b * P;
@@ -1057,11 +1056,33 @@ static int validate_prompts(const Model* m, const int32_t* prompts, int n, int P
   return sot_index;
 }
 
-static SearchParams search_params(const Model* m, const int32_t* prompts, int n, int K, int P, int sot_index, const b2w_gen_opts& o) {
-  const b2w_config& c = m->cfg;
+// Checks the options of a generate call against the model; returns K, the rows per chunk (beams, or independent hypotheses).
+static int check_gen_opts(const b2w_config& c, const b2w_gen_opts& o) {
+  B2W_CHECK(o.beam_size >= 1 && o.beam_size <= kMaxBeam, "beam_size must be in 1..16");
+  B2W_CHECK(o.num_hypotheses >= 1 && o.num_hypotheses <= kMaxBeam, "num_hypotheses must be in 1..16");
+  B2W_CHECK(o.beam_size == 1 || o.num_hypotheses <= o.beam_size, "num_hypotheses must be <= beam_size");
+  B2W_CHECK(o.max_length >= 1 && o.max_length <= c.n_text_ctx, "max_length must be in 1..n_text_ctx");
+  B2W_CHECK(o.sampling_topk == 0 || o.sampling_topk == 1, "sampling_topk must be 0 (full vocabulary) or 1 (argmax)");
+  B2W_CHECK(o.patience > 0 && o.repetition_penalty > 0, "patience and repetition_penalty must be positive");
+  return o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
+}
+
+// The always-suppressed tokens of a generate call, over the padded vocabulary (the padding columns are suppressed too).
+static std::vector<uint8_t> suppress_mask(const b2w_config& c, int vpad, const b2w_gen_opts& o) {
+  std::vector<uint8_t> mask(vpad, 0);
+  for (int i = c.n_vocab; i < vpad; ++i) mask[i] = 1;
+  for (int i = 0; i < o.n_suppress_tokens; ++i) {
+    const int t = o.suppress_tokens[i];
+    if (t >= 0 && t < c.n_vocab) mask[t] = 1;
+  }
+  return mask;
+}
+
+static SearchParams search_params(const b2w_config& c, int vpad, const int32_t* prompts, int n, int K, int P, int sot_index,
+                                  const b2w_gen_opts& o) {
   const bool beam = o.beam_size > 1;
   SearchParams sp{};
-  sp.n_vocab = c.n_vocab; sp.vpad = m->vpad; sp.B = n; sp.K = K;
+  sp.n_vocab = c.n_vocab; sp.vpad = vpad; sp.B = n; sp.K = K;
   sp.mode = beam ? 0 : 1;
   sp.ncand = beam ? 2 * K : 1;
   sp.max_steps = o.max_length - P; sp.prompt_len = P;
@@ -1082,7 +1103,9 @@ static SearchParams search_params(const Model* m, const int32_t* prompts, int n,
   sp.seed = o.seed;
   sp.want_no_speech_first = (o.return_no_speech_prob && sot_index == P - 1) ? 1 : 0;
   sp.fake_logits = o.debug_fake_logits;
-  B2W_CHECK(sp.max_finished <= kMaxFinished, "beam_size * patience is too large");
+  B2W_CHECK(sp.max_finished <= kMaxFinishTarget, "beam_size * patience is too large");
+  // a chunk stops at max_finished, but the step that reaches it can finish up to K hypotheses: all must have a slot
+  B2W_CHECK(!beam || sp.max_finished + K - 1 <= kMaxFinished, "beam_size * patience is too large");
   return sp;
 }
 
@@ -1307,9 +1330,9 @@ static void collect_hypotheses(Model* m, int chunk0, int n, int K, const b2w_gen
 static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_t* prompts, int P, const b2w_gen_opts& o,
                            int32_t* out_ids, int32_t* out_lens, float* out_scores, float* out_ns) {
   const int K = o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
-  const int sot_index = validate_prompts(m, prompts + (size_t)chunk0 * P, n, P);
+  const int sot_index = validate_prompts(m->cfg, prompts + (size_t)chunk0 * P, n, P);
   for (int b = 0; b < n; ++b) out_ns[chunk0 + b] = 0.f;
-  const SearchParams sp = search_params(m, prompts + (size_t)chunk0 * P, n, K, P, sot_index, o);
+  const SearchParams sp = search_params(m->cfg, m->vpad, prompts + (size_t)chunk0 * P, n, K, P, sot_index, o);
   Step st = choose_step(m, n, K, sp.fake_logits);
   if (sp.max_steps <= 0) {
     const int num_hyp = std::max(1, o.num_hypotheses);
@@ -1658,22 +1681,10 @@ int b2w_generate(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t
     const b2w_gen_opts& o = *opts;
     B2W_CHECK(batch > 0 && prompt_len > 0, "empty batch or prompt");
     B2W_CHECK(o.debug_fake_logits || (enc && enc->e && enc->e->B == batch), "one prompt per encoder output row is required");
-    B2W_CHECK(o.beam_size >= 1 && o.beam_size <= kMaxBeam, "beam_size must be in 1..16");
-    B2W_CHECK(o.num_hypotheses >= 1 && o.num_hypotheses <= kMaxBeam, "num_hypotheses must be in 1..16");
-    B2W_CHECK(o.beam_size == 1 || o.num_hypotheses <= o.beam_size, "num_hypotheses must be <= beam_size");
-    B2W_CHECK(o.max_length >= 1 && o.max_length <= m->cfg.n_text_ctx, "max_length must be in 1..n_text_ctx");
-    B2W_CHECK(o.sampling_topk == 0 || o.sampling_topk == 1, "sampling_topk must be 0 (full vocabulary) or 1 (argmax)");
-    B2W_CHECK(o.patience > 0 && o.repetition_penalty > 0, "patience and repetition_penalty must be positive");
-    const int K = o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
+    const int K = check_gen_opts(m->cfg, o);
     const int group = std::max(1, kMaxRows / K);
-    // suppress mask
     {
-      std::vector<uint8_t> mask(m->vpad, 0);
-      for (int i = m->cfg.n_vocab; i < m->vpad; ++i) mask[i] = 1;
-      for (int i = 0; i < o.n_suppress_tokens; ++i) {
-        const int t = o.suppress_tokens[i];
-        if (t >= 0 && t < m->cfg.n_vocab) mask[t] = 1;
-      }
+      const std::vector<uint8_t> mask = suppress_mask(m->cfg, m->vpad, o);
       B2W_CUDA(cudaMemcpyAsync(m->d_suppress, mask.data(), m->vpad, cudaMemcpyHostToDevice, m->stream));
       B2W_CUDA(cudaStreamSynchronize(m->stream));
     }
@@ -2194,7 +2205,7 @@ int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts
     b2w_gen_opts_default(&o);
     o.beam_size = K;
     o.max_length = P + n_steps;
-    bind_step(m, st, e, 0, prompts, P, search_params(m, prompts, n, K, P, -1, o));
+    bind_step(m, st, e, 0, prompts, P, search_params(c, m->vpad, prompts, n, K, P, -1, o));
     // anc[r][j]: the slot that holds key j of row r.  Keys of the prompt sit in slot 0; relinked as search_update does.
     std::vector<uint8_t> anc((size_t)R * n_ctx, 0), prev;
     std::vector<RowInfo> rows(R);
@@ -2219,6 +2230,111 @@ int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts
                                  cudaMemcpyDeviceToHost, s));
       B2W_CUDA(cudaStreamSynchronize(s));  // rows / anc are rewritten for the next step
     }
+  });
+}
+
+static_assert(B2W_MAX_FINISHED == kMaxFinished, "public finished-slot count");
+
+int b2w_debug_search(int32_t device, b2w_search_desc* d) {
+  return guarded([&] {
+    B2W_CHECK(d && d->cfg && d->opts && d->prompt && d->logits && d->hist && d->anc && d->cum && d->done && d->fin_count &&
+                  d->fin_len && d->fin_score && d->fin_tok && d->cand_score && d->cand_tok && d->no_speech && d->tokens_in && d->pos,
+              "null argument");
+    const b2w_config& c = *d->cfg;
+    const b2w_gen_opts& o = *d->opts;
+    const int V = c.n_vocab, n_ctx = c.n_text_ctx, vpad = ceil_div(std::max(V, 1), 16) * 16;
+    B2W_CHECK(V >= 1 && vpad * (int)sizeof(float) <= 210 * 1024, "n_vocab must fit the in-shared-memory row search");
+    B2W_CHECK(n_ctx >= 1 && n_ctx <= B2W_MAX_TEXT_CTX, "n_text_ctx must be in 1..448");
+    for (int tok : {c.eot, c.sot, c.no_speech, c.no_timestamps, c.timestamp_begin})
+      B2W_CHECK(tok >= 0 && tok < V, "control token id out of range");
+    B2W_CHECK(c.n_suppress_begin >= 0 && c.n_suppress_begin <= 8, "n_suppress_begin must be in 0..8");
+    for (int i = 0; i < c.n_suppress_begin; ++i) B2W_CHECK(c.suppress_begin[i] >= 0 && c.suppress_begin[i] < V, "suppress_begin id out of range");
+    const int K = check_gen_opts(c, o);
+    B2W_CHECK(d->K == K, "K must be beam_size, or num_hypotheses when beam_size is 1");
+    B2W_CHECK(o.n_suppress_tokens >= 0 && (o.n_suppress_tokens == 0 || o.suppress_tokens), "suppress_tokens");
+    const int n = d->n, P = d->P, t = d->t, R = n * K;
+    B2W_CHECK(n >= 1 && (int64_t)n * K <= kMaxRows, "chunks x rows per chunk must be in 1..80");
+    B2W_CHECK(P >= 1 && P <= n_ctx, "prompt length");
+    const int sot_index = validate_prompts(c, d->prompt, 1, P);
+    B2W_CHECK(t >= 0 && t < o.max_length - P, "step must be one a generate call with max_length runs");
+    std::vector<int32_t> prompts((size_t)n * P);
+    for (int b = 0; b < n; ++b) std::copy(d->prompt, d->prompt + P, prompts.begin() + (size_t)b * P);
+    const SearchParams sp = search_params(c, vpad, prompts.data(), n, K, P, sot_index, o);
+    const bool beam = sp.mode == 0;
+    for (size_t i = 0; i < (size_t)R * t; ++i) B2W_CHECK(d->hist[i] >= 0 && d->hist[i] < V, "history token id out of range");
+    for (size_t i = 0; i < (size_t)R * (P - 1 + t); ++i) B2W_CHECK(d->anc[i] < K, "ancestry slot out of range");
+    for (int b = 0; b < n; ++b) {
+      B2W_CHECK(d->done[b] == 0 || d->done[b] == 1, "done is 0 or 1");
+      B2W_CHECK(d->fin_count[b] >= 0 && d->fin_count[b] <= kMaxFinished, "fin_count out of range");
+      // a live beam chunk has room for the K hypotheses the step can finish, as in every state a generate call reaches unless
+      // early exit (patience 1, length penalty 0) lets hypotheses pile up behind a live best one
+      B2W_CHECK(!beam || d->done[b] || d->fin_count[b] + K <= kMaxFinished, "a live chunk needs K free finished slots");
+    }
+    for (size_t i = 0; i < (size_t)n * kMaxFinished; ++i) B2W_CHECK(d->fin_len[i] >= -1 && d->fin_len[i] <= n_ctx, "fin_len out of range");
+    B2W_CHECK(d->n_done >= 0 && d->n_done <= n, "n_done must be in 0..n");
+    require_hopper(device);
+    DeviceGuard g(device);
+    search_configure();  // per-device kernel attributes (build_model does this for real models)
+    ScratchBufs hb;
+    const int pos = P - 1 + t, cur = pos & 1, nxt = cur ^ 1;
+    const int ncand = sp.ncand;
+    SearchBuffers sb;
+    SearchState state{t, d->n_done, cur, 0};
+    sb.state = hb.put<SearchState>(&state, 1);
+    sb.params = hb.put<SearchParams>(&sp, 1);
+    std::vector<RowInfo> rows(R);
+    for (int r = 0; r < R; ++r) rows[r] = RowInfo{r / K, r % K, pos, 0};
+    sb.rows = hb.put<RowInfo>(rows.data(), R);
+    sb.tokens_in = hb.put<int>(nullptr, 0, R);
+    std::vector<float> cum(2 * (size_t)R, 0.f);
+    std::copy(d->cum, d->cum + R, cum.begin() + (size_t)cur * R);
+    sb.cum = hb.put<float>(cum.data(), cum.size());
+    std::vector<int> hist(2 * (size_t)R * n_ctx, -1);
+    std::vector<uint8_t> anc(2 * (size_t)R * n_ctx, 0xFF);
+    for (int r = 0; r < R; ++r) {
+      std::copy(d->hist + (size_t)r * t, d->hist + (size_t)(r + 1) * t, hist.begin() + ((size_t)cur * R + r) * n_ctx);
+      std::copy(d->anc + (size_t)r * pos, d->anc + (size_t)(r + 1) * pos, anc.begin() + ((size_t)cur * R + r) * n_ctx);
+    }
+    sb.hist = hb.put<int>(hist.data(), hist.size());
+    sb.anc = hb.put<uint8_t>(anc.data(), anc.size());
+    sb.cand_score = hb.put<float>(nullptr, 0, (size_t)R * kMaxCand);
+    sb.cand_tok = hb.put<int>(nullptr, 0, (size_t)R * kMaxCand);
+    const std::vector<uint8_t> mask = suppress_mask(c, vpad, o);
+    sb.suppress = hb.put<uint8_t>(mask.data(), mask.size());
+    sb.done = hb.put<int>(d->done, n);
+    sb.fin_count = hb.put<int>(d->fin_count, n);
+    sb.fin_score = hb.put<float>(d->fin_score, (size_t)n * kMaxFinished);
+    sb.fin_len = hb.put<int>(d->fin_len, (size_t)n * kMaxFinished);
+    const std::vector<int> fin_tok((size_t)n * kMaxFinished * n_ctx, -1);
+    sb.fin_tok = hb.put<int>(fin_tok.data(), fin_tok.size());
+    sb.no_speech = hb.put<float>(nullptr, 0, n);
+    sb.row_margin = hb.put<float>(nullptr, 0, R);
+    sb.n_ctx = n_ctx;
+    // logits at the padded row stride the decoder writes, NaN in the padding so that a read of it shows
+    float* logits = hb.alloc<float>((size_t)R * vpad);
+    B2W_CUDA(cudaMemset(logits, 0xFF, (size_t)R * vpad * sizeof(float)));
+    B2W_CUDA(cudaMemcpy2D(logits, (size_t)vpad * 4, d->logits, (size_t)V * 4, (size_t)V * 4, R, cudaMemcpyHostToDevice));
+    search_rows(logits, R, vpad, sb, 0);
+    search_update(n, sb, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    B2W_CUDA(cudaMemcpy2D(d->cand_score, (size_t)ncand * 4, sb.cand_score, (size_t)kMaxCand * 4, (size_t)ncand * 4, R, cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemcpy2D(d->cand_tok, (size_t)ncand * 4, sb.cand_tok, (size_t)kMaxCand * 4, (size_t)ncand * 4, R, cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemcpy2D(d->hist, (size_t)(t + 1) * 4, sb.hist + (size_t)nxt * R * n_ctx, (size_t)n_ctx * 4, (size_t)(t + 1) * 4, R,
+                          cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemcpy2D(d->anc, (size_t)(pos + 1), sb.anc + (size_t)nxt * R * n_ctx, (size_t)n_ctx, (size_t)(pos + 1), R, cudaMemcpyDeviceToHost));
+    hook_get(d->cum, sb.cum + (size_t)nxt * R, (size_t)R * 4);
+    hook_get(d->tokens_in, sb.tokens_in, (size_t)R * 4);
+    hook_get(rows.data(), sb.rows, (size_t)R * sizeof(RowInfo));
+    for (int r = 0; r < R; ++r) d->pos[r] = rows[r].pos;
+    hook_get(d->done, sb.done, (size_t)n * 4);
+    hook_get(&state, sb.state, sizeof state);
+    d->n_done = state.n_done;
+    hook_get(d->fin_count, sb.fin_count, (size_t)n * 4);
+    hook_get(d->fin_len, sb.fin_len, (size_t)n * kMaxFinished * 4);
+    hook_get(d->fin_score, sb.fin_score, (size_t)n * kMaxFinished * 4);
+    B2W_CUDA(cudaMemcpy2D(d->fin_tok, (size_t)(t + 1) * 4, sb.fin_tok, (size_t)n_ctx * 4, (size_t)(t + 1) * 4, (size_t)n * kMaxFinished,
+                          cudaMemcpyDeviceToHost));
+    hook_get(d->no_speech, sb.no_speech, (size_t)n * 4);
   });
 }
 

@@ -74,6 +74,65 @@ class _GemvDesc(C.Structure):  # b2w_gemv_desc
     ]
 
 
+class _SearchDesc(C.Structure):  # b2w_search_desc
+    _fields_ = [
+        ("cfg", C.POINTER(_Config)), ("opts", C.POINTER(_GenOpts)), ("prompt", C.c_void_p), ("P", C.c_int32), ("n", C.c_int32),
+        ("K", C.c_int32), ("t", C.c_int32), ("logits", C.c_void_p), ("hist", C.c_void_p), ("anc", C.c_void_p), ("cum", C.c_void_p),
+        ("done", C.c_void_p), ("fin_count", C.c_void_p), ("fin_len", C.c_void_p), ("fin_score", C.c_void_p), ("fin_tok", C.c_void_p),
+        ("cand_score", C.c_void_p), ("cand_tok", C.c_void_p), ("no_speech", C.c_void_p), ("tokens_in", C.c_void_p), ("pos", C.c_void_p),
+        ("n_done", C.c_int32),
+    ]
+
+
+MAX_FINISHED = 48  # include/b200whisper.h B2W_MAX_FINISHED: finished-hypothesis slots per chunk
+
+
+def _make_config(dims: WhisperDims, tokens: SpecialTokens) -> _Config:
+    cfg = _Config()
+    for k in ("n_mels", "n_audio_ctx", "n_audio_state", "n_audio_head", "n_audio_layer", "n_vocab", "n_text_ctx",
+              "n_text_state", "n_text_head", "n_text_layer"):
+        setattr(cfg, k, getattr(dims, k))
+    for k in ("eot", "sot", "lang_begin", "num_languages", "translate", "transcribe", "sot_lm", "sot_prev",
+              "no_speech", "no_timestamps", "timestamp_begin"):
+        setattr(cfg, k, getattr(tokens, k))
+    begin = [220, tokens.eot]
+    cfg.n_suppress_begin = len(begin)
+    for i, t in enumerate(begin):
+        cfg.suppress_begin[i] = t
+    return cfg
+
+
+def _gen_opts(lib, n_text_ctx: int, *, beam_size: int = 5, patience: float = 1, num_hypotheses: int = 1, length_penalty: float = 1,
+              repetition_penalty: float = 1, no_repeat_ngram_size: int = 0, max_length: int = 448, return_scores: bool = False,
+              return_no_speech_prob: bool = False, max_initial_timestamp_index: int = 50, suppress_blank: bool = True,
+              suppress_tokens: Optional[Sequence[int]] = (-1,), sampling_topk: int = 1, sampling_temperature: float = 1, seed: int = 0,
+              fake_logits: bool = False) -> Tuple[_GenOpts, np.ndarray]:
+    """b2w_gen_opts of Whisper.generate's keyword arguments, and the suppress-id array it points to (keep it alive).  Negative
+    suppress_tokens (the -1 that faster-whisper expands to the model's list itself) are dropped."""
+    sup = [int(t) for t in (suppress_tokens or []) if int(t) >= 0]
+    sup_arr = np.asarray(sorted(set(sup)), dtype=np.int32)
+    o = _GenOpts()
+    lib.b2w_gen_opts_default(C.byref(o))
+    o.beam_size = int(beam_size)
+    o.patience = float(patience)
+    o.num_hypotheses = int(num_hypotheses)
+    o.length_penalty = float(length_penalty)
+    o.repetition_penalty = float(repetition_penalty)
+    o.no_repeat_ngram_size = int(no_repeat_ngram_size)
+    o.max_length = int(min(max_length, n_text_ctx))
+    o.return_scores = int(bool(return_scores))
+    o.return_no_speech_prob = int(bool(return_no_speech_prob))
+    o.max_initial_timestamp_index = int(max_initial_timestamp_index)
+    o.suppress_blank = int(bool(suppress_blank))
+    o.suppress_tokens = sup_arr.ctypes.data_as(C.POINTER(C.c_int32)) if sup_arr.size else None
+    o.n_suppress_tokens = int(sup_arr.size)
+    o.sampling_topk = int(sampling_topk)
+    o.sampling_temperature = float(sampling_temperature)
+    o.seed = int(seed)
+    o.debug_fake_logits = int(bool(fake_logits))
+    return o, sup_arr
+
+
 # dense GEMM epilogues (include/b200whisper.h B2W_EPI_*) and decode GEMM modes (B2W_GV_*)
 EPI_F16, EPI_GELU_F16, EPI_RESID_F32, EPI_GELU_POS_F32, EPI_F16_XKV, EPI_F32, EPI_QKV_CACHE = range(7)
 EPI_F16_OUT = (EPI_F16, EPI_GELU_F16, EPI_F16_XKV, EPI_QKV_CACHE)
@@ -87,7 +146,7 @@ ABI_SYMBOLS = (
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
     "b2w_detect_language", "b2w_align", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
-    "b2w_debug_step_logits", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
+    "b2w_debug_step_logits", "b2w_debug_search", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
 )
 
 
@@ -147,6 +206,7 @@ def load_library():
         lib.b2w_debug_fetch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
         lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                               C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.b2w_debug_search.argtypes = [C.c_int32, C.POINTER(_SearchDesc)]
         lib.b2w_vad_create.argtypes = [C.c_int32, C.POINTER(_Tensor), C.c_int32, C.POINTER(C.c_void_p)]
         lib.b2w_vad_destroy.argtypes = [C.c_void_p]
         lib.b2w_vad_destroy.restype = None
@@ -343,17 +403,7 @@ class Whisper:
             self._config_alignment_heads = read_alignment_heads(model_path, files)
         self.dims = dims
         self.tokens = tokens or special_tokens(dims.n_vocab)
-        cfg = _Config()
-        for k in ("n_mels", "n_audio_ctx", "n_audio_state", "n_audio_head", "n_audio_layer", "n_vocab", "n_text_ctx",
-                  "n_text_state", "n_text_head", "n_text_layer"):
-            setattr(cfg, k, getattr(dims, k))
-        for k in ("eot", "sot", "lang_begin", "num_languages", "translate", "transcribe", "sot_lm", "sot_prev",
-                  "no_speech", "no_timestamps", "timestamp_begin"):
-            setattr(cfg, k, getattr(self.tokens, k))
-        begin = [220, self.tokens.eot]
-        cfg.n_suppress_begin = len(begin)
-        for i, t in enumerate(begin):
-            cfg.suppress_begin[i] = t
+        cfg = _make_config(dims, self.tokens)
         self._keep = []
         tensors = []
         for name, arr in weights.items():
@@ -501,27 +551,12 @@ class Whisper:
             raise ValueError("the number of prompts must match the batch size of the encoder output")
         rep = self._replica_for(enc) if enc is not None else self._replicas[0]
         B = len(prompts)
-        sup = [int(t) for t in (suppress_tokens or []) if int(t) >= 0]
-        sup_arr = np.asarray(sorted(set(sup)), dtype=np.int32)
-        o = _GenOpts()
-        rep._lib.b2w_gen_opts_default(C.byref(o))
-        o.beam_size = int(beam_size)
-        o.patience = float(patience)
-        o.num_hypotheses = int(num_hypotheses)
-        o.length_penalty = float(length_penalty)
-        o.repetition_penalty = float(repetition_penalty)
-        o.no_repeat_ngram_size = int(no_repeat_ngram_size)
-        o.max_length = int(min(max_length, self.dims.n_text_ctx))
-        o.return_scores = int(bool(return_scores))
-        o.return_no_speech_prob = int(bool(return_no_speech_prob))
-        o.max_initial_timestamp_index = int(max_initial_timestamp_index)
-        o.suppress_blank = int(bool(suppress_blank))
-        o.suppress_tokens = sup_arr.ctypes.data_as(C.POINTER(C.c_int32)) if sup_arr.size else None
-        o.n_suppress_tokens = int(sup_arr.size)
-        o.sampling_topk = int(sampling_topk)
-        o.sampling_temperature = float(sampling_temperature)
-        o.seed = int(seed)
-        o.debug_fake_logits = int(bool(_fake_logits))
+        o, sup_arr = _gen_opts(rep._lib, self.dims.n_text_ctx, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
+                               length_penalty=length_penalty, repetition_penalty=repetition_penalty,
+                               no_repeat_ngram_size=no_repeat_ngram_size, max_length=max_length, return_scores=return_scores,
+                               return_no_speech_prob=return_no_speech_prob, max_initial_timestamp_index=max_initial_timestamp_index,
+                               suppress_blank=suppress_blank, suppress_tokens=suppress_tokens, sampling_topk=sampling_topk,
+                               sampling_temperature=sampling_temperature, seed=seed, fake_logits=_fake_logits)
         H = max(1, o.num_hypotheses)
         pr = np.ascontiguousarray(np.asarray(prompts, dtype=np.int32))
         ids = np.zeros((B, H, o.max_length), dtype=np.int32)
@@ -651,6 +686,10 @@ class Whisper:
                                                   _ptr(out)))
         return out
 
+    def debug_search(self, logits: np.ndarray, prompt: Sequence[int], t: int, **kw) -> Dict[str, np.ndarray]:
+        """One step of the on-device search on caller-supplied state (tests only); see ``debug_search``.  The generate options
+        (beam_size, suppress_tokens, ...) are taken as ``generate`` takes them."""
+        return debug_search(self.dims, self.tokens, logits, prompt, t, device=self._device_index[0], **kw)
 
     def debug_fetch(self, which: int, n: int, replica: int = 0) -> np.ndarray:
         """Decoder workspace buffer `which` of the last decode step as float32 (tests / tools only)."""
@@ -804,6 +843,54 @@ def debug_gemv_desc(x: np.ndarray, w: np.ndarray, *, mode: int, bias: Optional[n
     desc.xres, desc.ln_g, desc.ln_b, desc.xn = _ptr(xres), _ptr(ln_g), _ptr(ln_b), _ptr(xn)
     _check(lib.b2w_debug_gemv(device, impl, C.byref(desc)))
     return desc.path_out
+
+
+def debug_search(dims: WhisperDims, tokens: SpecialTokens, logits: np.ndarray, prompt: Sequence[int], t: int, *,
+                 hist: Optional[np.ndarray] = None, anc: Optional[np.ndarray] = None, cum: Optional[np.ndarray] = None,
+                 done: Optional[np.ndarray] = None, fin_count: Optional[np.ndarray] = None, fin_len: Optional[np.ndarray] = None,
+                 fin_score: Optional[np.ndarray] = None, n_done: int = 0, device: int = 0, **opts) -> Dict[str, np.ndarray]:
+    """One decode step of the on-device search (b2w_search_desc; tests only) for n chunks x K rows at step t.
+
+    logits [n, K, n_vocab]; hist [n, K, t] generated tokens; anc [n, K, P-1+t] self-KV slot ancestry; cum [n, K]; done and fin_count
+    [n]; fin_len / fin_score [n, MAX_FINISHED] (fin_len -1 = empty).  Missing state starts empty.  ``opts`` are generate's keyword
+    arguments.  Returns the state after the step: cand_score / cand_tok [n, K, ncand], no_speech [n], hist [n, K, t+1],
+    anc [n, K, P+t], cum, tokens_in, pos [n, K], done, fin_count, n_done, fin_len, fin_score, and fin_tok [n, MAX_FINISHED, t+1]
+    (-1 in slots the step did not write)."""
+    lib = load_library()
+    logits = np.ascontiguousarray(logits, np.float32)
+    n, K, V = logits.shape
+    prompt = np.ascontiguousarray(list(prompt), np.int32)
+    P = prompt.shape[0]
+    o, sup_arr = _gen_opts(lib, dims.n_text_ctx, **opts)
+    ncand = 2 * K if o.beam_size > 1 else 1
+
+    def state(x, shape, dtype, fill=0):
+        return np.full(shape, fill, dtype) if x is None else np.array(np.broadcast_to(np.asarray(x, dtype), shape), dtype)
+
+    hist_in = state(hist, (n, K, t), np.int32)
+    anc_in = state(anc, (n, K, P - 1 + t), np.uint8)
+    out = dict(
+        hist=np.zeros((n, K, t + 1), np.int32), anc=np.zeros((n, K, P + t), np.uint8), cum=state(cum, (n, K), np.float32),
+        done=state(done, (n,), np.int32), fin_count=state(fin_count, (n,), np.int32),
+        fin_len=state(fin_len, (n, MAX_FINISHED), np.int32, -1), fin_score=state(fin_score, (n, MAX_FINISHED), np.float32),
+        fin_tok=np.zeros((n, MAX_FINISHED, t + 1), np.int32), cand_score=np.zeros((n, K, ncand), np.float32),
+        cand_tok=np.zeros((n, K, ncand), np.int32), no_speech=np.zeros(n, np.float32), tokens_in=np.zeros((n, K), np.int32),
+        pos=np.zeros((n, K), np.int32))
+    # hist and anc are in / out with the step's extra column: the input is packed into the front of the output buffers
+    out["hist"].reshape(-1)[: hist_in.size] = hist_in.reshape(-1)
+    out["anc"].reshape(-1)[: anc_in.size] = anc_in.reshape(-1)
+    cfg = _make_config(dims, tokens)
+    d = _SearchDesc()
+    d.cfg, d.opts, d.prompt = C.pointer(cfg), C.pointer(o), _ptr(prompt)
+    d.P, d.n, d.K, d.t = P, n, K, int(t)
+    d.logits = _ptr(logits)
+    for k in ("hist", "anc", "cum", "done", "fin_count", "fin_len", "fin_score", "fin_tok", "cand_score", "cand_tok", "no_speech",
+              "tokens_in", "pos"):
+        setattr(d, k, _ptr(out[k]))
+    d.n_done = int(n_done)
+    _check(lib.b2w_debug_search(device, C.byref(d)))
+    out["n_done"] = d.n_done
+    return out
 
 
 def debug_gemv(x: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, device: int = 0):

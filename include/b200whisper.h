@@ -263,6 +263,38 @@ int b2w_debug_logits(b2w_model* m, b2w_encoded* e, const int32_t* tokens, int32_
 int b2w_debug_step_logits(b2w_model* m, b2w_encoded* e, const int32_t* prompts, int32_t P, int32_t n, int32_t K,
                           int32_t n_steps, const int32_t* tokens, const int32_t* parents, float* logits_out);
 
+/* Finished-hypothesis slots the search keeps per chunk (b2w_search_desc.fin_*). */
+#define B2W_MAX_FINISHED 48
+
+/* One step of the on-device search, the two kernels a decode step runs after the decoder (logits processors, log-softmax and
+ * row top-k, then the beam / greedy update), on state the caller supplies.  The search parameters and the suppress mask are
+ * derived from cfg, opts and prompt by the code b2w_generate uses.  Rows r = b * K + k (chunk b, slot k) sit at position
+ * P - 1 + t.  In / out arrays are read before the step and overwritten with the state after it. */
+typedef struct b2w_search_desc {
+  const b2w_config* cfg;       /* geometry and control tokens of the model */
+  const b2w_gen_opts* opts;    /* generate options; K must be beam_size, or num_hypotheses when beam_size is 1 */
+  const int32_t* prompt;       /* [P], the prompt of every chunk: it fixes the SOT index and whether timestamp rules apply */
+  int32_t P, n, K, t;          /* prompt length, chunks, rows per chunk, step (tokens generated so far) */
+  const float* logits;         /* [n*K][n_vocab] decoder output of the step */
+  int32_t* hist;               /* in [n*K][t], out [n*K][t+1]: generated tokens of each row, relinked to the parent and extended */
+  uint8_t* anc;                /* in [n*K][P-1+t], out [n*K][P+t]: self-KV slot of each position; the last is the row's parent */
+  float* cum;                  /* in / out [n*K] cumulative log-prob */
+  int32_t* done;               /* in / out [n] */
+  int32_t* fin_count;          /* in / out [n] */
+  int32_t* fin_len;            /* in / out [n][B2W_MAX_FINISHED]; -1 = empty.  Greedy rows: slot k >= 0 means row k finished */
+  float* fin_score;            /* in / out [n][B2W_MAX_FINISHED] cumulative log-prob */
+  int32_t* fin_tok;            /* out [n][B2W_MAX_FINISHED][t+1]: tokens of the slots this step wrote, -1 elsewhere */
+  float* cand_score;           /* out [n*K][ncand] each row's candidates, best first (ncand = 2K in beam search, else 1) */
+  int32_t* cand_tok;           /* out [n*K][ncand] */
+  float* no_speech;            /* out [n] (written when the step computes it) */
+  int32_t* tokens_in;          /* out [n*K] the token each row feeds at the next step */
+  int32_t* pos;                /* out [n*K] the rows' next position */
+  int32_t n_done;              /* in / out: chunks done (the device counter the host polls) */
+} b2w_search_desc;
+
+/* Run one search step as described.  Every argument is checked before anything runs on the device. */
+int b2w_debug_search(int32_t device, b2w_search_desc* desc);
+
 /* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 the
  * many-row step kernel's split-K partial tiles of its last GEMM phase [CTA][R][128], 2 the per-k-atom partials of its last row
  * statistics [d/64][R][2], 4 attention output [R][d], 5 GELU(hidden) [R][4d], 6 final LayerNorm output [R][d], 7 LayerNorm

@@ -463,7 +463,14 @@ class WhisperOracle:
 
     @staticmethod
     def gumbel_noise(seed: int, row: int, step: int, n: int) -> np.ndarray:
-        """Counter-based noise shared with the CUDA sampler (csrc/decode_search.cu: gumbel_u32)."""
+        """Counter-based noise shared with the CUDA sampler (csrc/search.cu: gumbel_u32)."""
+        # 23 random bits + 0.5 is exact in float32 and keeps u strictly inside (0, 1)
+        u = (WhisperOracle.gumbel_bits(seed, row, step, n).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 8388608.0)
+        return (-np.log(-np.log(u))).astype(np.float32)
+
+    @staticmethod
+    def gumbel_bits(seed: int, row: int, step: int, n: int) -> np.ndarray:
+        """The 23-bit integers u * 2^23 - 0.5 behind gumbel_noise, for token ids 0..n-1."""
         M = (1 << 64) - 1
         base = (seed * 0xBF58476D1CE4E5B9 + row * 0x94D049BB133111EB + step * 0xD6E8FEB86659FD93) & M
         with np.errstate(over="ignore"):
@@ -473,9 +480,7 @@ class WhisperOracle:
             x ^= x >> np.uint64(27)
             x = x * np.uint64(0x94D049BB133111EB)
             x ^= x >> np.uint64(31)
-        # 23 random bits + 0.5 is exact in float32 and keeps u strictly inside (0, 1)
-        u = ((x >> np.uint64(41)).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 8388608.0)
-        return (-np.log(-np.log(u))).astype(np.float32)
+        return x >> np.uint64(41)
 
     def _sample(self, logp_row: np.ndarray, topk: int, temperature: float, seed: int, row: int, step: int):
         """Random sampling as Gumbel-max over logp/T (distributionally equal to CT2's multinomial;

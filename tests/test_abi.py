@@ -57,6 +57,50 @@ def test_gemm_hooks_check_arguments_before_the_device():
         engine.debug_gemv_desc(np.zeros((81, 64), np.float16), w, mode=engine.GV_F32, out=np.zeros(81 * 128, np.float32), ldo=128)
 
 
+def test_search_hook_checks_arguments_before_the_device():
+    """Bad search-step descriptors are refused (ValueError) before anything touches a device, GPU or not."""
+    from faster_whisper_b200.config import special_tokens
+    from faster_whisper_b200.synthetic import custom_dims
+
+    dims = custom_dims(n_vocab=51865)
+    st = special_tokens(dims.n_vocab)
+    V = dims.n_vocab
+
+    def call(K=2, t=1, prompt=(st.sot, st.no_timestamps), **kw):
+        opts = dict(beam_size=2, max_length=20)
+        opts.update(kw)
+        return engine.debug_search(dims, st, np.zeros((1, K, V), np.float32), prompt, t, **opts)
+
+    with pytest.raises(ValueError, match="K must be"):
+        call(beam_size=3)
+    with pytest.raises(ValueError, match="beam_size must be in"):
+        call(K=17, beam_size=17)
+    with pytest.raises(ValueError, match="beam_size \\* patience"):
+        call(K=16, beam_size=16, patience=2.1)
+    with pytest.raises(ValueError, match="num_hypotheses must be <= beam_size"):
+        call(num_hypotheses=3)
+    with pytest.raises(ValueError, match="startoftranscript"):
+        call(prompt=(st.no_timestamps,))
+    with pytest.raises(ValueError, match="prompt token id"):
+        call(prompt=(st.sot, V))
+    with pytest.raises(ValueError, match="step must be"):
+        call(t=18)
+    with pytest.raises(ValueError, match="history token id"):
+        call(hist=[[[V], [0]]])
+    with pytest.raises(ValueError, match="ancestry slot"):
+        call(anc=2)
+    with pytest.raises(ValueError, match="done is 0 or 1"):
+        call(done=[2])
+    with pytest.raises(ValueError, match="K free finished slots"):
+        call(fin_count=[engine.MAX_FINISHED - 1])
+    with pytest.raises(ValueError, match="fin_len"):
+        call(fin_len=-2)
+    with pytest.raises(ValueError, match="n_done"):
+        engine.debug_search(dims, st, np.zeros((1, 2, V), np.float32), (st.sot,), 0, beam_size=2, n_done=2)
+    with pytest.raises(ValueError, match="chunks x rows"):
+        engine.debug_search(dims, st, np.zeros((6, 16, V), np.float32), (st.sot,), 0, beam_size=16)
+
+
 def test_no_cpu_fallback():
     if engine.device_count() > 0:
         pytest.skip("a GPU is present")
