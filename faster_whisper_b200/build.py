@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200whisper.so")
-SOURCES = ["mel.cu", "gemm.cu", "attention.cu", "encoder_misc.cu", "decode.cu", "dstep.cu", "bstep.cu", "search.cu", "vad.cu", "engine.cu"]
+SOURCES = ["mel.cu", "gemm.cu", "attention.cu", "encoder_misc.cu", "decode.cu", "dstep.cu", "bstep.cu", "search.cu", "align.cu", "vad.cu", "engine.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",

@@ -133,7 +133,27 @@ void no_speech_from_logits(const float* logits, int row_stride, int R, int rows_
 void lang_probs_from_logits(const float* logits, int row_stride, int B, int lang_begin, int n_lang, float* out, cudaStream_t s);
 // Whisper.align helpers (search.cu)
 void row_target_probs(const float* logits, int row_stride, int R, int n_vocab, const int* targets, float* out, cudaStream_t s);
-void align_probs(const __half* q, const DecBindings* bind, int layer, const int2* heads, int n_heads, float* out, int n_tok, int nf,
-                 int pos0, int R, int H, int T, int d, cudaStream_t s);
+// Row r of the pass writes out[rows[r].chunk][head][rows[r].pos][0..nf) of an [items][n_heads][n_tok][nf] capture, with the keys
+// of encoder chunk bind->chunk0 + rows[r].chunk.
+void align_probs(const __half* q, const DecBindings* bind, const RowInfo* rows, int layer, const int2* heads, int n_heads, float* out,
+                 int n_tok, int nf, int R, int H, int T, int d, cudaStream_t s);
+
+// ---- Whisper.align post-processing (align.cu) ----------------------------------------------------------------------------
+constexpr int kAlignMaxRows = 449;  // DTW rows (n_text + 1) the kernels take: more than a 448-position decoder can force
+
+// Items of one align group, all with the same strides.  Item b: items[b] = (n_tok, nf, row0, n_rows); its capture is
+// cap[b][n_heads][tok_stride][nf_stride], and the DTW runs over its rows row0 .. row0 + n_rows - 1 (n_rows = 0: no path).
+struct AlignBatch {
+  const float* cap;
+  double* stats;      // [items][n_heads][2][nf_stride]: mean, std over the tokens
+  double* cost;       // [items][row_stride][nf_stride]
+  const int4* items;
+  int n_heads, tok_stride, nf_stride, row_stride, width;
+  int2* pairs;        // [items][row_stride + nf_stride] (text index, frame index) from (0, 0)
+  int* n_pairs;       // [items]
+};
+void align_check(const AlignBatch& a);
+void align_cost(const AlignBatch& a, int n_items, cudaStream_t s);  // cap -> stats -> cost
+void align_dtw(const AlignBatch& a, int n_items, cudaStream_t s);   // cost -> pairs, n_pairs
 
 }  // namespace b2w

@@ -738,6 +738,7 @@ static int mel_frames(int64_t n_samples) { return (int)(1 + n_samples / 160); }
 
 // ---- decoder ----------------------------------------------------------------------------------------------------------------
 constexpr int kMaxRows = 80;
+constexpr size_t kCrossGroupCounters = 16 * 20 * 64;  // (chunk, head, query group) counters of the layered cross-attention
 
 static void ensure_decoder_ws(Model* m, int chunks, int slots) {
   const int dt = m->cfg.n_text_state, L = m->cfg.n_text_layer, n_ctx = m->cfg.n_text_ctx;
@@ -947,13 +948,13 @@ static void ensure_xpart(Model* m, size_t floats) {
   m->d_xpart_floats = floats;
 }
 
-// Whisper.align: the cross-attention probabilities of the alignment heads for the rows of one forced-decoding pass of one chunk,
-// row r written to out[head][pos0 + r][0..nf) of an [n_heads][n_tok][nf] buffer.
+// Whisper.align: the cross-attention probabilities of the alignment heads for the rows of forced-decoding passes, the row at
+// position p of chunk b (relative to the pass's first chunk) written to out[b][head][p][0..nf) of an [n][n_heads][n_tok][nf] buffer.
 struct AlignCapture {
   const int2* heads;
   int n_heads;
   float* out;
-  int n_tok, nf, pos0;
+  int n_tok, nf;
 };
 
 // The layered decoder step: one launch per GEMM / attention.  Needs ensure_xpart(m, xpart_floats(m, n_chunks, rows_per_chunk)).
@@ -965,7 +966,7 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
   const SearchBuffers& sb = m->sb;
   embed_ln(sb.tokens_in, sb.rows, m->tok_emb, m->dec_pos, nullptr, nullptr, m->d_x, m->d_xn, R, dt, c.n_vocab, s);
   B2W_CHECK(m->d_xpart_floats >= xpart_floats(m, n_chunks, rows_per_chunk), "cross-attention partial buffer");
-  B2W_CHECK((size_t)n_chunks * H * ds_xqgroups(rows_per_chunk) <= 16 * 20 * 64, "cross-attention group counters");
+  B2W_CHECK((size_t)n_chunks * H * ds_xqgroups(rows_per_chunk) <= kCrossGroupCounters, "cross-attention group counters");
   for (int l = 0; l < L; ++l) {
     const DecLayerW& W = m->dec[l];
     __half* kc = m->kcache + (size_t)l * m->kv_elems;
@@ -983,7 +984,7 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     GvArgs q;
     q.x = m->d_xn; q.W = W.wq_x; q.bias = W.bq_x; q.R = R; q.N = dt; q.K = dt; q.mode = GV_F16; q.out_h = m->d_q;
     gv(m, q);
-    if (cap) align_probs(m->d_q, m->d_bind, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, cap->pos0, R, H, 1500, dt, s);
+    if (cap) align_probs(m->d_q, m->d_bind, sb.rows, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, R, H, 1500, dt, s);
     DStepArgs xa{};
     xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
     xa.H = H; xa.T = 1500; xa.d = dt; xa.rows_per_chunk = rows_per_chunk; xa.n_chunks = n_chunks;
@@ -1009,15 +1010,17 @@ static void logits_gemm(Model* m, int R) {
   gv(m, a);
 }
 
-// Forced decoding of tokens[b * stride + i], i < n_tok, for chunks chunk0 .. chunk0+n of `e`, in passes of max(1, 80 / n)
-// positions; every row writes self-KV slot 0 of `slots`.  The slot ancestry must be zero: clear_anc zeroes it, unless the caller
-// already has.  When `cap` is set, every pass captures the alignment heads' cross-attention (cap->pos0 is set per pass).
+static int forced_positions_per_pass(int n_chunks) { return std::max(1, kMaxRows / n_chunks); }
+
+// Forced decoding of tokens[b * stride + i], i < n_tok, for chunks chunk0 .. chunk0+n of `e`, in passes of
+// forced_positions_per_pass(n) positions; every row writes self-KV slot 0 of `slots`.  The slot ancestry must be zero: clear_anc
+// zeroes it, unless the caller already has.  When `cap` is set, every pass captures the alignment heads' cross-attention.
 // After each pass's decoder layers, on_pass(i0, i1) may run logits_gemm: row b * (i1 - i0) + (i - i0) holds position i of chunk b.
 template <typename F>
 static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int n_tok, int slots,
-                          bool clear_anc, AlignCapture* cap, F&& on_pass) {
+                          bool clear_anc, const AlignCapture* cap, F&& on_pass) {
   if (clear_anc) B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * slots * m->cfg.n_text_ctx, m->stream));
-  const int per_pass = std::max(1, kMaxRows / n);
+  const int per_pass = forced_positions_per_pass(n);
   for (int i0 = 0; i0 < n_tok; i0 += per_pass) {
     const int i1 = std::min(n_tok, i0 + per_pass), rpc = i1 - i0, R = n * rpc;
     std::vector<RowInfo> rows(R);
@@ -1032,7 +1035,6 @@ static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const i
     B2W_CUDA(cudaStreamSynchronize(m->stream));  // host vectors go out of scope
     bind_encoded(m, e, chunk0);
     ensure_xpart(m, xpart_floats(m, n, rpc));
-    if (cap) cap->pos0 = i0;
     decoder_layers(m, n, rpc, slots, cap);
     on_pass(i0, i1);
   }
@@ -1719,60 +1721,150 @@ int b2w_detect_language(b2w_model* h, b2w_encoded* enc, float* probs) {
   });
 }
 
-// ---- Whisper.align: host-side post-processing (fp64) ------------------------------------------------------------------------
-static void median_filter_rows(std::vector<double>& x, int rows, int cols, int width) {
-  const int pad = width / 2;
-  if (pad == 0 || cols <= pad) return;
-  std::vector<double> row(cols + 2 * pad), win(width), out(cols);
-  for (int r = 0; r < rows; ++r) {
-    double* p = x.data() + (size_t)r * cols;
-    for (int i = 0; i < pad; ++i) {  // reflect (edge sample not repeated)
-      row[pad - 1 - i] = p[i + 1];
-      row[pad + cols + i] = p[cols - 2 - i];
-    }
-    for (int i = 0; i < cols; ++i) row[pad + i] = p[i];
-    for (int i = 0; i < cols; ++i) {
-      for (int k = 0; k < width; ++k) win[k] = row[i + k];
-      std::nth_element(win.begin(), win.begin() + pad, win.end());
-      out[i] = win[pad];
-    }
-    for (int i = 0; i < cols; ++i) p[i] = out[i];
+// ---- Whisper.align --------------------------------------------------------------------------------------------------------
+// Capture of one align group (items x alignment heads x positions x frames, fp32): 320 heads of a 155-position, 1500-frame
+// chunk take 300 MB.  A single item may exceed it.
+constexpr size_t kAlignCaptureBytes = (size_t)2 << 30;
+
+static int align_frames(int num_frames) { return std::max(1, std::min(1500, num_frames / 2)); }
+
+// Checks an item's forced sequence, start_sequence + <|notimestamps|> + text + <|endoftext|>, against the model.
+static void check_align_sequence(const b2w_config& c, const int32_t* start, int n_start, const int32_t* text, int n_text) {
+  if (n_start + n_text + 2 > c.n_text_ctx) throw Error("align: start sequence + text exceed the decoder context", true);
+  for (int i = 0; i < n_start + n_text; ++i) {
+    const int t = i < n_start ? start[i] : text[i - n_start];
+    if (t < 0 || t >= c.n_vocab) throw Error("align: token id out of range", true);
   }
 }
 
-// monotone minimal-cost path through cost[N][M]; moves diagonal / down / right with the reference tie rule
-static void dtw_path(const std::vector<double>& c, int N, int M, std::vector<int>& ti, std::vector<int>& fi) {
-  const double inf = std::numeric_limits<double>::infinity();
-  std::vector<double> cost((size_t)(N + 1) * (M + 1), inf);
-  std::vector<int8_t> trace((size_t)(N + 1) * (M + 1), -1);
-  auto at = [&](int i, int j) { return (size_t)i * (M + 1) + j; };
-  cost[0] = 0.0;
-  for (int j = 1; j <= M; ++j)
-    for (int i = 1; i <= N; ++i) {
-      const double c0 = cost[at(i - 1, j - 1)], c1 = cost[at(i - 1, j)], c2 = cost[at(i, j - 1)];
-      double best;
-      int8_t t;
-      if (c0 < c1 && c0 < c2) { best = c0; t = 0; }
-      else if (c1 < c0 && c1 < c2) { best = c1; t = 1; }
-      else { best = c2; t = 2; }
-      cost[at(i, j)] = c[(size_t)(i - 1) * M + (j - 1)] + best;
-      trace[at(i, j)] = t;
+struct AlignItem {
+  const int32_t* text;
+  int n_text, nf;
+  float* probs;             // host [n_text]: probability of each text token at the position that predicts it
+  std::vector<int2> pairs;  // the DTW path (text index, frame index); none when n_text = 0
+};
+
+// Aligns items[k] against chunk chunk0 + k of `e` (arguments already checked).  Consecutive items form groups whose padded
+// sequences fit one pass of kMaxRows rows, so that every pass reads each chunk's cross-attention K/V once: splitting a long
+// sequence over the passes of a group would re-read every chunk's K/V in each pass, which costs more than the weights it shares
+// (an item longer than a pass is a group of its own).  The group's cross-attention counters and capture must fit too.  A group's
+// sequences are padded with <|endoftext|> to its longest, and the padded positions' capture and probabilities are never read
+// (attention is causal, so they do not change the real rows).  Per group: the forced decode with the capture and the text-token
+// probabilities, then the cost matrix and the DTW on the device.  Pairs, counts and probabilities come back with one copy each
+// and one synchronise.
+static void align_run(Model* m, const Encoded* e, int chunk0, const int32_t* start, int n_start, std::vector<AlignItem>& items, int width) {
+  const b2w_config& c = m->cfg;
+  cudaStream_t s = m->stream;
+  const int n_heads = (int)m->align_heads.size(), n_items = (int)items.size();
+  B2W_CHECK(n_heads > 0, "no alignment heads");
+  struct Group {
+    int i0, n, T, nf;            // first item, items, padded positions, frames of the capture
+    size_t tp_off, pair_off;     // offsets of the group's probabilities and pair slots in the call's buffers
+  };
+  std::vector<Group> groups;
+  size_t tp_total = 0, pair_total = 0, cap_max = 0, stats_max = 0, cost_max = 0;
+  for (int i0 = 0; i0 < n_items;) {
+    Group g{i0, 0, 0, 0, tp_total, pair_total};
+    while (i0 + g.n < n_items) {
+      const int n = g.n + 1, T = std::max(g.T, n_start + items[i0 + g.n].n_text + 2), nf = std::max(g.nf, items[i0 + g.n].nf);
+      const bool fits = n * T <= kMaxRows && (size_t)n * c.n_text_head * ds_xqgroups(forced_positions_per_pass(n)) <= kCrossGroupCounters &&
+                        (size_t)n * n_heads * T * nf * sizeof(float) <= kAlignCaptureBytes;
+      if (g.n > 0 && !fits) break;
+      g.n = n, g.T = T, g.nf = nf;
     }
-  for (int j = 0; j <= M; ++j) trace[at(0, j)] = 2;
-  for (int i = 0; i <= N; ++i) trace[at(i, 0)] = 1;
-  int i = N, j = M;
-  ti.clear();
-  fi.clear();
-  while (i > 0 || j > 0) {
-    ti.push_back(i - 1);
-    fi.push_back(j - 1);
-    const int8_t t = trace[at(i, j)];
-    if (t == 0) { --i; --j; }
-    else if (t == 1) --i;
-    else --j;
+    const size_t row_stride = g.T - n_start - 1;  // n_text + 1 of the group's longest text
+    tp_total += (size_t)g.n * g.T;
+    pair_total += (size_t)g.n * (row_stride + g.nf);
+    cap_max = std::max(cap_max, (size_t)g.n * n_heads * g.T * g.nf);
+    stats_max = std::max(stats_max, (size_t)g.n * n_heads * 2 * g.nf);
+    cost_max = std::max(cost_max, (size_t)g.n * row_stride * g.nf);
+    groups.push_back(g);
+    i0 += g.n;
   }
-  std::reverse(ti.begin(), ti.end());
-  std::reverse(fi.begin(), fi.end());
+  // row of position i of the group's item b in its forced decode: passes of p positions of every item, pass-major
+  auto row_of = [](const Group& g, int b, int i) {
+    const int p = forced_positions_per_pass(g.n), i0 = i / p * p, rpc = std::min(g.T, i0 + p) - i0;
+    return g.tp_off + (size_t)g.n * i0 + (size_t)b * rpc + (i - i0);
+  };
+  std::vector<int> targets(tp_total, -1);  // position n_start + t predicts text token t
+  std::vector<int4> desc(n_items);
+  for (const Group& g : groups)
+    for (int b = 0; b < g.n; ++b) {
+      const AlignItem& it = items[g.i0 + b];
+      for (int t = 0; t < it.n_text; ++t) targets[row_of(g, b, n_start + t)] = it.text[t];
+      desc[g.i0 + b] = make_int4(n_start + it.n_text + 2, it.nf, n_start, it.n_text > 0 ? it.n_text + 1 : 0);
+    }
+  int max_n = 0;
+  for (const Group& g : groups) max_n = std::max(max_n, g.n);
+  prepare_decode(m, const_cast<Encoded*>(e), max_n, 1);
+  if (!m->d_align_heads) {
+    m->d_align_heads = dalloc<int2>(n_heads);
+    B2W_CUDA(cudaMemcpy(m->d_align_heads, m->align_heads.data(), n_heads * sizeof(int2), cudaMemcpyHostToDevice));
+  }
+  struct PoolBufs {  // returned to the model's pool when the call ends
+    Model* m;
+    std::vector<std::pair<void*, size_t>> v;
+    void* get(size_t bytes) {
+      bytes = std::max<size_t>(bytes, 1);
+      v.emplace_back(m->pool_get(bytes), bytes);
+      return v.back().first;
+    }
+    ~PoolBufs() {
+      for (auto& x : v) m->pool_put(x.first, x.second);
+    }
+  } pb{m, {}};
+  float* d_cap = static_cast<float*>(pb.get(cap_max * sizeof(float)));
+  double* d_stats = static_cast<double*>(pb.get(stats_max * sizeof(double)));
+  double* d_cost = static_cast<double*>(pb.get(cost_max * sizeof(double)));
+  int* d_targets = static_cast<int*>(pb.get(tp_total * sizeof(int)));
+  float* d_tp = static_cast<float*>(pb.get(tp_total * sizeof(float)));
+  int2* d_pairs = static_cast<int2*>(pb.get(pair_total * sizeof(int2)));
+  int* d_counts = static_cast<int*>(pb.get(n_items * sizeof(int)));
+  int4* d_items = static_cast<int4*>(pb.get(n_items * sizeof(int4)));
+  B2W_CUDA(cudaMemcpyAsync(d_targets, targets.data(), tp_total * sizeof(int), cudaMemcpyHostToDevice, s));
+  B2W_CUDA(cudaMemcpyAsync(d_items, desc.data(), n_items * sizeof(int4), cudaMemcpyHostToDevice, s));
+  B2W_CUDA(cudaMemsetAsync(d_tp, 0, tp_total * sizeof(float), s));
+  B2W_CUDA(cudaMemsetAsync(d_counts, 0, n_items * sizeof(int), s));
+  for (const Group& g : groups) {
+    bool any = false;
+    for (int b = 0; b < g.n; ++b) any = any || items[g.i0 + b].n_text > 0;
+    if (!any) continue;
+    std::vector<int32_t> toks((size_t)g.n * g.T, c.eot);
+    for (int b = 0; b < g.n; ++b) {
+      const AlignItem& it = items[g.i0 + b];
+      int32_t* p = toks.data() + (size_t)b * g.T;
+      std::copy(start, start + n_start, p);
+      p[n_start] = c.no_timestamps;
+      std::copy(it.text, it.text + it.n_text, p + n_start + 1);
+    }
+    const AlignCapture cap{m->d_align_heads, n_heads, d_cap, g.T, g.nf};
+    forced_decode(m, e, chunk0 + g.i0, g.n, toks.data(), g.T, g.T, 1, true, &cap, [&](int i0, int i1) {
+      const int R = g.n * (i1 - i0);
+      const size_t off = g.tp_off + (size_t)g.n * i0;
+      logits_gemm(m, R);
+      row_target_probs(m->d_logits, m->vpad, R, c.n_vocab, d_targets + off, d_tp + off, s);
+    });
+    const int row_stride = g.T - n_start - 1;
+    const AlignBatch ab{d_cap, d_stats, d_cost, d_items + g.i0, n_heads, g.T, g.nf, row_stride, width, d_pairs + g.pair_off, d_counts + g.i0};
+    align_cost(ab, g.n, s);
+    align_dtw(ab, g.n, s);
+  }
+  std::vector<int> counts(n_items);
+  std::vector<float> tp(tp_total);
+  std::vector<int2> pairs(pair_total);
+  B2W_CUDA(cudaMemcpyAsync(counts.data(), d_counts, n_items * sizeof(int), cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(tp.data(), d_tp, tp_total * sizeof(float), cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(pairs.data(), d_pairs, pair_total * sizeof(int2), cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaStreamSynchronize(s));
+  for (const Group& g : groups) {
+    const size_t slot = (size_t)(g.T - n_start - 1) + g.nf;
+    for (int b = 0; b < g.n; ++b) {
+      AlignItem& it = items[g.i0 + b];
+      for (int t = 0; t < it.n_text; ++t) it.probs[t] = tp[row_of(g, b, n_start + t)];
+      const int2* p = pairs.data() + g.pair_off + b * slot;
+      it.pairs.assign(p, p + counts[g.i0 + b]);
+    }
+  }
 }
 
 int b2w_model_set_alignment_heads(b2w_model* h, const int32_t* layer_head_pairs, int32_t n_pairs) {
@@ -1797,84 +1889,60 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
               int32_t capacity_pairs, int32_t* n_pairs_out, float* text_token_probs_out) {
   return guarded(h, [&](Model* m) {
     B2W_CHECK(enc && enc->e && start_sequence && n_pairs_out && n_start >= 1 && n_text >= 0, "bad arguments");
-    const b2w_config& c = m->cfg;
     Encoded* e = enc->e;
     if (batch_index < 0 || batch_index >= e->B) throw Error("align: batch index out of range", true);
     if (median_filter_width < 1 || median_filter_width % 2 == 0) throw Error("align: median_filter_width must be odd", true);
     *n_pairs_out = 0;
     if (n_text == 0) return;
     B2W_CHECK(text_tokens && text_token_probs_out && (alignments_out || capacity_pairs == 0), "bad arguments");
-    // forced sequence: start_sequence + <|notimestamps|> + text + <|endoftext|>
-    std::vector<int32_t> seq(start_sequence, start_sequence + n_start);
-    seq.push_back(c.no_timestamps);
-    const int n_head_rows = (int)seq.size();
-    seq.insert(seq.end(), text_tokens, text_tokens + n_text);
-    seq.push_back(c.eot);
-    const int n_tok = (int)seq.size();
-    if (n_tok > c.n_text_ctx) throw Error("align: start sequence + text exceed the decoder context", true);
-    for (int t : seq)
-      if (t < 0 || t >= c.n_vocab) throw Error("align: token id out of range", true);
-    const int nf = std::max(1, std::min(1500, (int)num_frames / 2));
-    cudaStream_t s = m->stream;
-    prepare_decode(m, e, 1, 1);
-    const int n_heads = (int)m->align_heads.size();
-    B2W_CHECK(n_heads > 0, "no alignment heads");
-    if (!m->d_align_heads) {
-      m->d_align_heads = dalloc<int2>(n_heads);
-      B2W_CUDA(cudaMemcpy(m->d_align_heads, m->align_heads.data(), n_heads * sizeof(int2), cudaMemcpyHostToDevice));
+    check_align_sequence(m->cfg, start_sequence, n_start, text_tokens, n_text);
+    std::vector<AlignItem> items{AlignItem{text_tokens, n_text, align_frames(num_frames), text_token_probs_out, {}}};
+    align_run(m, e, batch_index, start_sequence, n_start, items, median_filter_width);
+    const std::vector<int2>& p = items[0].pairs;
+    *n_pairs_out = (int32_t)p.size();
+    if ((int)p.size() > capacity_pairs) throw Error("align: alignment buffer too small", true);
+    for (size_t i = 0; i < p.size(); ++i) {
+      alignments_out[2 * i] = p[i].x;
+      alignments_out[2 * i + 1] = p[i].y;
     }
-    const size_t n_att = (size_t)n_heads * n_tok * nf;
-    float* d_att = reinterpret_cast<float*>(m->pool_get(n_att * sizeof(float)));
-    int* d_targets = reinterpret_cast<int*>(m->pool_get((size_t)n_tok * sizeof(int)));
-    float* d_tp = reinterpret_cast<float*>(m->pool_get((size_t)n_tok * sizeof(float)));
-    std::vector<int> targets(n_tok, -1);
-    for (int t = 0; t < n_text; ++t) targets[n_head_rows - 1 + t] = text_tokens[t];  // position p predicts token p + 1
-    B2W_CUDA(cudaMemcpyAsync(d_targets, targets.data(), (size_t)n_tok * sizeof(int), cudaMemcpyHostToDevice, s));
-    B2W_CUDA(cudaMemsetAsync(d_tp, 0, (size_t)n_tok * sizeof(float), s));
-    AlignCapture cap{m->d_align_heads, n_heads, d_att, n_tok, nf, 0};
-    forced_decode(m, e, batch_index, 1, seq.data(), n_tok, n_tok, 1, true, &cap, [&](int i0, int i1) {
-      logits_gemm(m, i1 - i0);
-      row_target_probs(m->d_logits, m->vpad, i1 - i0, c.n_vocab, d_targets + i0, d_tp + i0, s);
-    });
-    std::vector<float> att(n_att), tp(n_tok);
-    B2W_CUDA(cudaMemcpyAsync(att.data(), d_att, n_att * sizeof(float), cudaMemcpyDeviceToHost, s));
-    B2W_CUDA(cudaMemcpyAsync(tp.data(), d_tp, (size_t)n_tok * sizeof(float), cudaMemcpyDeviceToHost, s));
-    B2W_CUDA(cudaStreamSynchronize(s));
-    m->pool_put(d_att, n_att * sizeof(float));
-    m->pool_put(d_targets, (size_t)n_tok * sizeof(int));
-    m->pool_put(d_tp, (size_t)n_tok * sizeof(float));
-    for (int t = 0; t < n_text; ++t) text_token_probs_out[t] = tp[n_head_rows - 1 + t];
-    // per head: normalise over the token axis (population std), median filter along time; then the head mean
-    std::vector<double> mean_w((size_t)n_tok * nf, 0.0), w((size_t)n_tok * nf);
-    for (int hd = 0; hd < n_heads; ++hd) {
-      const float* a = att.data() + (size_t)hd * n_tok * nf;
-      for (int f = 0; f < nf; ++f) {
-        double mu = 0.0, var = 0.0;
-        for (int t = 0; t < n_tok; ++t) mu += a[(size_t)t * nf + f];
-        mu /= n_tok;
-        for (int t = 0; t < n_tok; ++t) {
-          const double dlt = a[(size_t)t * nf + f] - mu;
-          var += dlt * dlt;
-        }
-        const double sd = std::sqrt(var / n_tok);
-        for (int t = 0; t < n_tok; ++t) w[(size_t)t * nf + f] = (a[(size_t)t * nf + f] - mu) / sd;
+  });
+}
+
+int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequence, int32_t n_start, const int32_t* text_tokens,
+                    const int32_t* text_offsets, const int32_t* num_frames, int32_t median_filter_width, int32_t* alignments_out,
+                    int32_t capacity_pairs, int32_t* pair_offsets_out, float* text_token_probs_out) {
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && start_sequence && n_start >= 1 && text_offsets && num_frames && pair_offsets_out, "bad arguments");
+    Encoded* e = enc->e;
+    const int B = e->B;
+    if (median_filter_width < 1 || median_filter_width % 2 == 0) throw Error("align: median_filter_width must be odd", true);
+    if (text_offsets[0] != 0) throw Error("align: text_offsets must start at 0", true);
+    for (int b = 0; b < B; ++b)
+      if (text_offsets[b + 1] < text_offsets[b]) throw Error("align: text_offsets must not decrease", true);
+    B2W_CHECK(text_offsets[B] == 0 || (text_tokens && text_token_probs_out), "bad arguments");
+    std::vector<AlignItem> items(B);
+    int64_t need = 0;
+    for (int b = 0; b < B; ++b) {
+      AlignItem& it = items[b];
+      it.n_text = text_offsets[b + 1] - text_offsets[b];
+      it.nf = align_frames(num_frames[b]);
+      if (it.n_text == 0) continue;
+      it.text = text_tokens + text_offsets[b];
+      it.probs = text_token_probs_out + text_offsets[b];
+      check_align_sequence(m->cfg, start_sequence, n_start, it.text, it.n_text);
+      need += it.n_text + 1 + it.nf;  // the longest path through (n_text + 1) x nf cells
+    }
+    if (need > capacity_pairs) throw Error("align: alignment buffer too small: it needs sum(n_text + 1 + nf) pairs", true);
+    B2W_CHECK(need == 0 || alignments_out, "bad arguments");
+    if (need > 0) align_run(m, e, 0, start_sequence, n_start, items, median_filter_width);
+    pair_offsets_out[0] = 0;
+    for (int b = 0; b < B; ++b) {
+      const std::vector<int2>& p = items[b].pairs;
+      for (size_t i = 0; i < p.size(); ++i) {
+        alignments_out[2 * ((size_t)pair_offsets_out[b] + i)] = p[i].x;
+        alignments_out[2 * ((size_t)pair_offsets_out[b] + i) + 1] = p[i].y;
       }
-      median_filter_rows(w, n_tok, nf, median_filter_width);
-      for (size_t i = 0; i < w.size(); ++i) mean_w[i] += w[i];
-    }
-    // rows of the inputs that predict text + eot (drop the start-sequence rows and the eot input row: the consumer indexes
-    // word boundaries up to n_text, transcribe.py:1744-1746), negated, DTW
-    const int n_rows = n_text + 1;
-    std::vector<double> cost((size_t)n_rows * nf);
-    for (int t = 0; t < n_rows; ++t)
-      for (int f = 0; f < nf; ++f) cost[(size_t)t * nf + f] = -mean_w[(size_t)(n_start + t) * nf + f] / n_heads;
-    std::vector<int> ti, fi;
-    dtw_path(cost, n_rows, nf, ti, fi);
-    *n_pairs_out = (int32_t)ti.size();
-    if ((int)ti.size() > capacity_pairs) throw Error("align: alignment buffer too small", true);
-    for (size_t i = 0; i < ti.size(); ++i) {
-      alignments_out[2 * i] = ti[i];
-      alignments_out[2 * i + 1] = fi[i];
+      pair_offsets_out[b + 1] = pair_offsets_out[b] + (int32_t)p.size();
     }
   });
 }
@@ -2125,6 +2193,57 @@ int b2w_debug_gemv(int32_t device, int32_t impl, b2w_gemv_desc* d) {
       hook_get(d->xres, a.xres, (size_t)R * N * 4);
       hook_get(d->xn, a.xn_out, (size_t)R * N * 2);
     }
+  });
+}
+
+int b2w_debug_align_cost(int32_t device, const float* capture, int32_t n_heads, int32_t n_tok, int32_t nf, int32_t n_start,
+                         int32_t n_text, int32_t median_filter_width, double* cost_out) {
+  return guarded([&] {
+    B2W_CHECK(capture && cost_out, "null argument");
+    B2W_CHECK(n_heads >= 1 && n_heads <= 32 * 32, "n_heads must be in 1..1024");
+    B2W_CHECK(nf >= 1 && nf <= 1500, "nf must be in 1..1500");
+    B2W_CHECK(n_tok >= 1 && n_tok <= B2W_MAX_TEXT_CTX, "n_tok must be in 1..448");
+    B2W_CHECK(n_start >= 0 && n_text >= 0 && n_start + n_text + 1 <= n_tok, "the kept rows n_start .. n_start + n_text must be tokens");
+    if (median_filter_width < 1 || median_filter_width % 2 == 0) throw Error("align: median_filter_width must be odd", true);
+    const AlignBatch shape{nullptr, nullptr, nullptr, nullptr, n_heads, n_tok, nf, n_text + 1, median_filter_width, nullptr, nullptr};
+    align_check(shape);
+    require_hopper(device);
+    DeviceGuard g(device);
+    const size_t n_cap = (size_t)n_heads * n_tok * nf, n_cost = (size_t)(n_text + 1) * nf;
+    const int4 item = make_int4(n_tok, nf, n_start, n_text + 1);
+    ScratchBufs sb;
+    AlignBatch a = shape;
+    a.cap = sb.put<float>(capture, n_cap);
+    a.stats = sb.alloc<double>((size_t)n_heads * 2 * nf);
+    a.cost = sb.alloc<double>(n_cost);
+    a.items = sb.put<int4>(&item, 1);
+    align_cost(a, 1, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    B2W_CUDA(cudaMemcpy(cost_out, a.cost, n_cost * sizeof(double), cudaMemcpyDeviceToHost));
+  });
+}
+
+int b2w_debug_dtw(int32_t device, const double* cost, int32_t N, int32_t M, int32_t* pairs_out, int32_t capacity_pairs,
+                  int32_t* n_pairs_out) {
+  return guarded([&] {
+    B2W_CHECK(cost && pairs_out && n_pairs_out, "null argument");
+    B2W_CHECK(N >= 1 && N <= kAlignMaxRows && M >= 1 && M <= 1500, "cost must be 1..449 rows x 1..1500 frames");
+    if (capacity_pairs < N + M) throw Error("align: alignment buffer too small: it needs N + M pairs", true);
+    const AlignBatch shape{nullptr, nullptr, nullptr, nullptr, 1, 1, M, N, 1, nullptr, nullptr};
+    align_check(shape);
+    require_hopper(device);
+    DeviceGuard g(device);
+    const int4 item = make_int4(N + 1, M, 0, N);
+    ScratchBufs sb;
+    AlignBatch a = shape;
+    a.cost = sb.put<double>(cost, (size_t)N * M);
+    a.items = sb.put<int4>(&item, 1);
+    a.pairs = sb.alloc<int2>(N + M);
+    a.n_pairs = sb.alloc<int>(1);
+    align_dtw(a, 1, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    B2W_CUDA(cudaMemcpy(n_pairs_out, a.n_pairs, sizeof(int), cudaMemcpyDeviceToHost));
+    B2W_CUDA(cudaMemcpy(pairs_out, a.pairs, (size_t)*n_pairs_out * sizeof(int2), cudaMemcpyDeviceToHost));
   });
 }
 

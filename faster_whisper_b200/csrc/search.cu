@@ -579,20 +579,22 @@ void row_target_probs(const float* logits, int row_stride, int R, int n_vocab, c
 }
 
 // Cross-attention probabilities of the alignment heads of one layer for forced-decoding rows (Whisper.align): CTA per
-// (alignment head, row); softmax over all T encoder positions, the first nf written out as out[head][pos0 + row][t].
-// K rows are stored with their 16-byte chunks at chunk ^ (t & 7) (gemm.cu EPI_F16_XKV).
-__global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restrict__ q, const DecBindings* __restrict__ bind, int layer,
-                                                          const int2* __restrict__ heads, float* __restrict__ out, int n_tok, int nf,
-                                                          int pos0, int H, int T, int d) {
+// (alignment head, row); softmax over all T encoder positions, the first nf written out as out[chunk][head][pos][t] for the
+// row's chunk (relative to bind->chunk0) and position.  K rows are stored with their 16-byte chunks at chunk ^ (t & 7)
+// (gemm.cu EPI_F16_XKV).
+__global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restrict__ q, const DecBindings* __restrict__ bind,
+                                                          const RowInfo* __restrict__ rows, int layer, const int2* __restrict__ heads,
+                                                          float* __restrict__ out, int n_tok, int nf, int H, int T, int d) {
   const int2 lh = heads[blockIdx.x];
   if (lh.x != layer) return;
   __shared__ float qs[64];
   __shared__ float sc[1536];
   __shared__ float red[32];
   const int r = blockIdx.y, h = lh.y, tid = threadIdx.x;
+  const RowInfo ri = rows[r];
   const DecBindings bd = *bind;
   const long long per = (long long)bd.B_total * H * T * 64;
-  const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + (((long long)bd.chunk0 * H + h) * T) * 64;
+  const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + (((long long)(bd.chunk0 + ri.chunk) * H + h) * T) * 64;
   if (tid < 64) qs[tid] = __half2float(q[(long long)r * d + h * 64 + tid]) * 0.125f;
   __syncthreads();
   float mx = -INFINITY;
@@ -619,13 +621,13 @@ __global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restri
     sm += e;
   }
   sm = block_sum(sm, red);
-  float* o = out + ((long long)blockIdx.x * n_tok + pos0 + r) * nf;
+  float* o = out + (((long long)ri.chunk * gridDim.x + blockIdx.x) * n_tok + ri.pos) * nf;
   for (int t = tid; t < nf; t += 256) o[t] = sc[t] / sm;
 }
-void align_probs(const __half* q, const DecBindings* bind, int layer, const int2* heads, int n_heads, float* out, int n_tok, int nf,
-                 int pos0, int R, int H, int T, int d, cudaStream_t s) {
+void align_probs(const __half* q, const DecBindings* bind, const RowInfo* rows, int layer, const int2* heads, int n_heads, float* out,
+                 int n_tok, int nf, int R, int H, int T, int d, cudaStream_t s) {
   B2W_CHECK(T <= 1536, "align_probs: encoder length");
-  align_probs_kernel<<<dim3(n_heads, R), 256, 0, s>>>(q, bind, layer, heads, out, n_tok, nf, pos0, H, T, d);
+  align_probs_kernel<<<dim3(n_heads, R), 256, 0, s>>>(q, bind, rows, layer, heads, out, n_tok, nf, H, T, d);
   B2W_LAUNCHED();
 }
 

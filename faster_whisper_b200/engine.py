@@ -144,9 +144,9 @@ ABI_SYMBOLS = (
     "b2w_last_error", "b2w_abi_version", "b2w_device_count", "b2w_model_create", "b2w_model_destroy",
     "b2w_model_info", "b2w_model_sync", "b2w_logmel", "b2w_logmel_frames", "b2w_encode", "b2w_encode_audio",
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
-    "b2w_detect_language", "b2w_align", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
+    "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
-    "b2w_debug_step_logits", "b2w_debug_search", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
+    "b2w_debug_step_logits", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
 )
 
 
@@ -192,6 +192,8 @@ def load_library():
         lib.b2w_detect_language.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b2w_align.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]
+        lib.b2w_align_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         lib.b2w_model_set_alignment_heads.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         lib.b2w_timing_enable.argtypes = [C.c_void_p, C.c_int32]
         lib.b2w_timing_reset.argtypes = [C.c_void_p]
@@ -207,6 +209,9 @@ def load_library():
         lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                               C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b2w_debug_search.argtypes = [C.c_int32, C.POINTER(_SearchDesc)]
+        lib.b2w_debug_align_cost.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p]
+        lib.b2w_debug_dtw.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
         lib.b2w_vad_create.argtypes = [C.c_int32, C.POINTER(_Tensor), C.c_int32, C.POINTER(C.c_void_p)]
         lib.b2w_vad_destroy.argtypes = [C.c_void_p]
         lib.b2w_vad_destroy.restype = None
@@ -602,19 +607,21 @@ class Whisper:
         start = np.ascontiguousarray(list(start_sequence), dtype=np.int32)
         if len(text_tokens) != enc.shape[0]:
             raise ValueError("align: one text token list per batch item is required")
-        results = []
-        for b, toks in enumerate(text_tokens):
-            nf = int(num_frames[b] if isinstance(num_frames, (list, tuple)) else num_frames)
-            toks = np.ascontiguousarray(list(toks), dtype=np.int32)
-            cap = len(toks) + nf // 2 + 2
-            pairs = np.zeros((cap, 2), np.int32)
-            probs = np.zeros(max(1, len(toks)), np.float32)
-            n_pairs = C.c_int32(0)
-            with rep.lock:
-                _check(rep._lib.b2w_align(rep.handle, enc._handle, b, _ptr(start), len(start), _ptr(toks), len(toks), nf, int(median_filter_width),
-                                          _ptr(pairs), cap, C.byref(n_pairs), _ptr(probs)))
-            results.append(WhisperAlignmentResult([(int(a), int(t)) for a, t in pairs[: n_pairs.value]], [float(p) for p in probs[: len(toks)]]))
-        return results
+        B = enc.shape[0]
+        texts = [np.asarray(list(t), dtype=np.int32) for t in text_tokens]
+        frames = np.ascontiguousarray([int(num_frames[b] if isinstance(num_frames, (list, tuple)) else num_frames) for b in range(B)], np.int32)
+        offsets = np.zeros(B + 1, np.int32)
+        offsets[1:] = np.cumsum([len(t) for t in texts])
+        toks = np.ascontiguousarray(np.concatenate(texts) if offsets[-1] else np.zeros(1, np.int32), dtype=np.int32)
+        cap = int(sum(len(t) + max(1, min(1500, nf // 2)) + 1 for t, nf in zip(texts, frames) if len(t)))
+        pairs = np.zeros((max(1, cap), 2), np.int32)
+        pair_offsets = np.zeros(B + 1, np.int32)
+        probs = np.zeros(max(1, int(offsets[-1])), np.float32)
+        with rep.lock:
+            _check(rep._lib.b2w_align_batch(rep.handle, enc._handle, _ptr(start), len(start), _ptr(toks), _ptr(offsets), _ptr(frames),
+                                            int(median_filter_width), _ptr(pairs), cap, _ptr(pair_offsets), _ptr(probs)))
+        return [WhisperAlignmentResult([tuple(p) for p in pairs[pair_offsets[b]:pair_offsets[b + 1]].tolist()],
+                                       probs[offsets[b]:offsets[b + 1]].tolist()) for b in range(B)]
 
     def set_alignment_heads(self, heads=None):
         """(layer, head) pairs from a converted model's config.json ``alignment_heads``; None restores the default."""
@@ -891,6 +898,28 @@ def debug_search(dims: WhisperDims, tokens: SpecialTokens, logits: np.ndarray, p
     _check(lib.b2w_debug_search(device, C.byref(d)))
     out["n_done"] = d.n_done
     return out
+
+
+def debug_align_cost(capture: np.ndarray, n_start: int, n_text: int, median_filter_width: int = 7, device: int = 0) -> np.ndarray:
+    """The DTW cost matrix [n_text + 1, nf] (float64) of Whisper.align from a float32 capture [n_heads, n_tok, nf] (tests only)."""
+    lib = load_library()
+    cap = np.ascontiguousarray(capture, np.float32)
+    n_heads, n_tok, nf = cap.shape
+    out = np.zeros((max(0, n_text) + 1, nf), np.float64)
+    _check(lib.b2w_debug_align_cost(device, _ptr(cap), n_heads, n_tok, nf, n_start, n_text, median_filter_width, _ptr(out)))
+    return out
+
+
+def debug_dtw(cost: np.ndarray, capacity: Optional[int] = None, device: int = 0) -> List[Tuple[int, int]]:
+    """The DTW path of Whisper.align through a float64 cost [N, M] as (row, frame) pairs (tests only)."""
+    lib = load_library()
+    c = np.ascontiguousarray(cost, np.float64)
+    N, M = c.shape
+    cap = N + M if capacity is None else capacity
+    pairs = np.zeros((max(1, cap), 2), np.int32)
+    n = C.c_int32(0)
+    _check(lib.b2w_debug_dtw(device, _ptr(c), N, M, _ptr(pairs), cap, C.byref(n)))
+    return [(int(a), int(b)) for a, b in pairs[: n.value]]
 
 
 def debug_gemv(x: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, device: int = 0):

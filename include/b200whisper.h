@@ -140,6 +140,17 @@ int b2w_align(b2w_model* m, b2w_encoded* e, int32_t batch_index, const int32_t* 
               int32_t median_filter_width, int32_t* alignments_out, int32_t capacity_pairs,
               int32_t* n_pairs_out, float* text_token_probs_out);
 
+/* b2w_align for every batch item of e in one call, item for item with b2w_align's contract.  Item b's text is
+ * text_tokens[text_offsets[b] .. text_offsets[b+1]) (text_offsets[0] = 0, never decreasing) and its frames num_frames[b];
+ * an item with no text gets no pairs.  Its pairs are alignments_out[pair_offsets_out[b] .. pair_offsets_out[b+1]) and its
+ * probabilities text_token_probs_out[text_offsets[b] .. text_offsets[b+1]).  capacity_pairs must be at least the sum of
+ * n_text + 1 + min(1500, num_frames/2) over the items with text.  Items are decoded in groups of consecutive chunks; the
+ * cost matrix and the DTW run on the device, and the host waits once at the end. */
+int b2w_align_batch(b2w_model* m, b2w_encoded* e, const int32_t* start_sequence, int32_t n_start,
+                    const int32_t* text_tokens, const int32_t* text_offsets, const int32_t* num_frames,
+                    int32_t median_filter_width, int32_t* alignments_out, int32_t capacity_pairs,
+                    int32_t* pair_offsets_out, float* text_token_probs_out);
+
 /* config.json "alignment_heads" of a converted model (transcribe.py:700-710 reads the model directory): n_pairs
  * (layer, head) pairs; n_pairs = 0 restores the default (every head of the last half of the decoder layers). */
 int b2w_model_set_alignment_heads(b2w_model* m, const int32_t* layer_head_pairs, int32_t n_pairs);
@@ -294,6 +305,18 @@ typedef struct b2w_search_desc {
 
 /* Run one search step as described.  Every argument is checked before anything runs on the device. */
 int b2w_debug_search(int32_t device, b2w_search_desc* desc);
+
+/* The cost matrix of Whisper.align from a capture[n_heads][n_tok][nf] of cross-attention probabilities: per head and frame
+ * normalised over the tokens (population std), median-filtered along time (odd width, reflect padding, none when
+ * nf <= width/2), averaged over the heads and negated, for rows n_start .. n_start + n_text: cost_out[n_text + 1][nf].
+ * Every argument is checked before anything runs on the device. */
+int b2w_debug_align_cost(int32_t device, const float* capture, int32_t n_heads, int32_t n_tok, int32_t nf, int32_t n_start,
+                         int32_t n_text, int32_t median_filter_width, double* cost_out);
+
+/* The DTW path of Whisper.align through cost[N][M] (N <= 449, M <= 1500): n_pairs_out (text index, frame index) pairs
+ * from (0, 0) to (N - 1, M - 1) in pairs_out, which must hold N + M.  Arguments are checked before any device work. */
+int b2w_debug_dtw(int32_t device, const double* cost, int32_t N, int32_t M, int32_t* pairs_out, int32_t capacity_pairs,
+                  int32_t* n_pairs_out);
 
 /* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 the
  * many-row step kernel's split-K partial tiles of its last GEMM phase [CTA][R][128], 2 the per-k-atom partials of its last row
