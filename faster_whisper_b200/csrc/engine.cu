@@ -1457,11 +1457,16 @@ struct b2w_vad {
   ScratchBufs weights;        // every weight buffer and the LSTM state
   VadWeights w;
   const float *w_hh = nullptr, *dec_w = nullptr, *dec_b = nullptr;
-  float* state = nullptr;     // h [128] then c [128], carried from block to block
-  int64_t block = 32768;      // windows per block; the buffers below take (512 + 512 + 128 + 1) floats = 4.6 KB per window
+  int64_t block = 32768;      // windows per block, summed over the streams of a launch; the buffers below take
+                              // (512 + 512 + 128 + 1) floats = 4.6 KB per window, and 64 + 256 floats and a table entry per stream
   int64_t cap = 0;            // windows the block buffers hold
+  int64_t cap_streams = 0;    // streams they hold
   std::unique_ptr<ScratchBufs> bufs;
   float *pcm = nullptr, *gx = nullptr, *H = nullptr, *probs = nullptr;
+  float* states = nullptr;    // per stream: h [128] then c [128], carried from launch to launch
+  VadSlice* slices = nullptr; // the launch's stream table
+  std::vector<VadSlice> host_slices;
+  std::vector<float> host_probs;
   cudaEvent_t ev[4] = {};
   double ms[3] = {0, 0, 0};   // last call: window kernel, recurrence, decoder
   ~b2w_vad() {  // the buffers are freed after this body, once the stream has drained
@@ -2487,7 +2492,6 @@ int b2w_vad_create(int32_t device, const b2w_tensor* tensors, int32_t n_tensors,
     v->w_hh = raw("lstm.w_hh");
     v->dec_w = raw("decoder.weight");
     v->dec_b = raw("decoder.bias");
-    v->state = sb.put<float>(nullptr, 0, 256);
     *out = v.release();
   });
 }
@@ -2503,53 +2507,114 @@ int b2w_vad_set_block(b2w_vad* v, int64_t windows) {
   });
 }
 
+// Windows of stream i per launch: the block's windows split evenly over the streams that still have windows left (a launch
+// takes as long as its longest slice), what a short stream leaves over going to the longer ones.
+static void vad_plan_launch(int64_t block, const std::vector<int64_t>& left, std::vector<int64_t>& take) {
+  std::vector<int> order;
+  for (int i = 0; i < (int)left.size(); ++i)
+    if (left[i] > 0) order.push_back(i);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return left[a] < left[b]; });
+  std::fill(take.begin(), take.end(), 0);
+  int64_t budget = block;
+  for (size_t k = 0; k < order.size(); ++k) {
+    const int64_t t = std::min(left[order[k]], budget / (int64_t)(order.size() - k));
+    take[order[k]] = t;
+    budget -= t;
+  }
+}
+
 int b2w_vad_probs(b2w_vad* v, const float* pcm, int64_t n_samples, float* probs_out, int64_t capacity) {
+  return b2w_vad_probs_multi(v, &pcm, &n_samples, 1, probs_out, capacity);
+}
+
+int b2w_vad_probs_multi(b2w_vad* v, const float* const* pcm, const int64_t* n_samples, int32_t n_streams, float* probs_out,
+                        int64_t capacity) {
   return guarded([&] {
-    B2W_CHECK(pcm && probs_out, "null argument");
-    B2W_CHECK(n_samples > 0 && n_samples % 512 == 0, "the number of samples must be a positive multiple of 512");
-    const int64_t N = n_samples / 512;
-    B2W_CHECK(capacity >= N, "output buffer too small: one probability per 512 samples");
+    B2W_CHECK(pcm && n_samples && probs_out, "null argument");
+    B2W_CHECK(n_streams >= 1, "at least one stream");
+    int64_t total = 0;
+    for (int i = 0; i < n_streams; ++i) {
+      B2W_CHECK(pcm[i], "null argument");
+      B2W_CHECK(n_samples[i] > 0 && n_samples[i] % 512 == 0, "the number of samples must be a positive multiple of 512");
+      total += n_samples[i] / 512;
+    }
+    B2W_CHECK(capacity >= total, "output buffer too small: one probability per 512 samples");
     B2W_CHECK(v, "null VAD handle");
     std::lock_guard<std::mutex> lk(v->mu);
     DeviceGuard g(v->device);
     cudaStream_t s = v->stream;
-    const int64_t nb_max = std::min(v->block, N);
-    if (v->cap < nb_max) {
-      v->bufs.reset();
-      v->cap = 0;
-      std::unique_ptr<ScratchBufs> b(new ScratchBufs);
-      v->pcm = b->alloc<float>((size_t)(64 + 512 * nb_max));
-      v->gx = b->alloc<float>((size_t)(512 * nb_max));
-      v->H = b->alloc<float>((size_t)(128 * nb_max));
-      v->probs = b->alloc<float>((size_t)nb_max);
-      v->bufs = std::move(b);
-      v->cap = nb_max;
+    const int S = n_streams;
+    std::vector<int64_t> left(S), done(S, 0), out0(S), take(S);  // per stream: windows to go, done, first output, this launch
+    for (int64_t i = 0, o = 0; i < S; ++i) {
+      left[i] = n_samples[i] / 512;
+      out0[i] = o;
+      o += left[i];
     }
-    B2W_CUDA(cudaMemsetAsync(v->state, 0, 256 * sizeof(float), s));
+    const int64_t nb_max = std::min(v->block, total);
+    if (v->cap < nb_max || v->cap_streams < S) {
+      const int64_t cap = std::max(v->cap, nb_max), cap_streams = std::max<int64_t>(v->cap_streams, S);
+      v->bufs.reset();
+      v->cap = v->cap_streams = 0;
+      std::unique_ptr<ScratchBufs> b(new ScratchBufs);
+      v->pcm = b->alloc<float>((size_t)(64 * std::min(cap, cap_streams) + 512 * cap));
+      v->gx = b->alloc<float>((size_t)(512 * cap));
+      v->H = b->alloc<float>((size_t)(128 * cap));
+      v->probs = b->alloc<float>((size_t)cap);
+      v->states = b->alloc<float>((size_t)(256 * cap_streams));
+      v->slices = b->alloc<VadSlice>((size_t)std::min(cap, cap_streams));
+      v->bufs = std::move(b);
+      v->cap = cap;
+      v->cap_streams = cap_streams;
+    }
+    v->host_probs.resize((size_t)nb_max);
     for (double& m : v->ms) m = 0;
-    for (int64_t n0 = 0; n0 < N; n0 += nb_max) {
-      const int nb = (int)std::min(nb_max, N - n0);
-      // the 64 samples before the block (zeros before the audio), then the block
-      if (n0 == 0) {
-        B2W_CUDA(cudaMemsetAsync(v->pcm, 0, 64 * sizeof(float), s));
-        B2W_CUDA(cudaMemcpyAsync(v->pcm + 64, pcm, (size_t)nb * 512 * 4, cudaMemcpyHostToDevice, s));
-      } else {
-        B2W_CUDA(cudaMemcpyAsync(v->pcm, pcm + n0 * 512 - 64, (64 + (size_t)nb * 512) * 4, cudaMemcpyHostToDevice, s));
+    for (int64_t remaining = total; remaining > 0;) {
+      vad_plan_launch(nb_max, left, take);
+      // the launch's table and PCM: per slice the 64 samples before it (left to the kernel at the start of a stream), then its
+      // windows
+      auto& tab = v->host_slices;
+      tab.clear();
+      int64_t w = 0, p = 0;
+      for (int i = 0; i < S; ++i) {
+        if (take[i] == 0) continue;
+        VadSlice sl{};
+        sl.pcm0 = p;
+        sl.w0 = (int32_t)w;
+        sl.nb = (int32_t)take[i];
+        sl.stream = i;
+        sl.first = done[i] == 0;
+        sl.last = done[i] + take[i] == n_samples[i] / 512;
+        tab.push_back(sl);
+        const int64_t n_pcm = 512 * take[i];
+        if (sl.first)
+          B2W_CUDA(cudaMemcpyAsync(v->pcm + p + 64, pcm[i], (size_t)n_pcm * 4, cudaMemcpyHostToDevice, s));
+        else
+          B2W_CUDA(cudaMemcpyAsync(v->pcm + p, pcm[i] + done[i] * 512 - 64, (size_t)(64 + n_pcm) * 4, cudaMemcpyHostToDevice, s));
+        w += take[i];
+        p += 64 + n_pcm;
       }
+      const int nb = (int)w, n_slices = (int)tab.size();
+      B2W_CUDA(cudaMemcpyAsync(v->slices, tab.data(), tab.size() * sizeof(VadSlice), cudaMemcpyHostToDevice, s));
       B2W_CUDA(cudaEventRecord(v->ev[0], s));
-      vad_windows(v->w, v->pcm, nb, n0 + nb == N, v->gx, s);
+      vad_windows(v->w, v->pcm, v->slices, n_slices, nb, v->gx, s);
       B2W_CUDA(cudaEventRecord(v->ev[1], s));
-      vad_recurrence(v->w_hh, v->gx, nb, v->state, v->state + 128, v->H, s);
+      vad_recurrence(v->w_hh, v->slices, n_slices, v->gx, v->states, v->H, s);
       B2W_CUDA(cudaEventRecord(v->ev[2], s));
       vad_decoder(v->H, v->dec_w, v->dec_b, nb, v->probs, s);
       B2W_CUDA(cudaEventRecord(v->ev[3], s));
-      B2W_CUDA(cudaMemcpyAsync(probs_out + n0, v->probs, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+      B2W_CUDA(cudaMemcpyAsync(v->host_probs.data(), v->probs, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
       B2W_CUDA(cudaStreamSynchronize(s));
       for (int i = 0; i < 3; ++i) {
         float ms = 0.f;
         B2W_CUDA(cudaEventElapsedTime(&ms, v->ev[i], v->ev[i + 1]));
         v->ms[i] += ms;
       }
+      for (const VadSlice& sl : tab) {
+        memcpy(probs_out + out0[sl.stream] + done[sl.stream], v->host_probs.data() + sl.w0, (size_t)sl.nb * 4);
+        done[sl.stream] += sl.nb;
+        left[sl.stream] -= sl.nb;
+      }
+      remaining -= nb;
     }
   });
 }

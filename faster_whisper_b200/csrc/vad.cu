@@ -1,10 +1,12 @@
 // Silero VAD v6 (16 kHz) on the GPU, fp32 throughout (faster_whisper_b200/silero.py states the graph):
 //   vad_window_kernel      per window, parallel: PCM -> 576-sample input -> reflect pad -> STFT magnitude (frames 1..4)
 //                          -> 4 x conv+ReLU -> LSTM input projection Gx[n][512] = W_ih x + b_ih + b_hh
-//   vad_recurrence_kernel  the LSTM over all windows of a block in one launch: one cluster of 4 CTAs, each owning 32 hidden
-//                          units (their 4 x 32 rows of W_hh live in registers); h goes to every CTA through DSMEM, one cluster
-//                          barrier per step
+//   vad_recurrence_kernel  the LSTM over all windows of a block in one launch: one cluster of 4 CTAs per stream slice, each
+//                          CTA owning 32 hidden units (their 4 x 32 rows of W_hh live in registers); h goes to every CTA of the
+//                          cluster through DSMEM, one cluster barrier per step; clusters never wait for each other
 //   vad_decoder_kernel     per window, parallel: p = sigmoid(w . relu(h) + b)
+// A launch serves several independent audio streams: its windows are the concatenation of one slice per stream (VadSlice), and
+// a window's arithmetic does not depend on where in the launch it lands, so every stream gets the bits it gets alone.
 // No TF32 or fp16: a probability is compared with thresholds, so error becomes a moved speech boundary.
 #include "vad.h"
 
@@ -54,21 +56,52 @@ static __device__ __forceinline__ void conv_relu(const float* __restrict__ in, f
     for (int t = 0; t < LOUT; ++t) out[((w0 + w) * COUT + co) * LOUT + t] = fmaxf(acc[w][t] + b, 0.f);
 }
 
-__global__ void __launch_bounds__(kThreads) vad_window_kernel(VadWeights wts, const float* __restrict__ pcm, int nb, int last_is_tail,
+// The slice holding window n of the launch (slices are in window order and none is empty).
+static __device__ __forceinline__ int vad_find_slice(const VadSlice* __restrict__ slices, int n_slices, int n) {
+  int lo = 0, hi = n_slices - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&slices[mid].w0) <= n) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kThreads) vad_window_kernel(VadWeights wts, const float* __restrict__ pcm,
+                                                              const VadSlice* __restrict__ slices, int n_slices, int nb,
                                                               float* __restrict__ gx) {
   extern __shared__ float smem[];
+  __shared__ int64_t win_pcm[kTile];  // where window w of the tile starts in pcm (its 64 context samples first), -1: none
+  __shared__ int win_flags[kTile];    // 1: context is zero (the stream's first window), 2: tail is zero (its last window)
   float* A = smem;
   float* B = smem + kBufA;
   const int n0 = blockIdx.x * kTile;
-  // 1. inputs: window w is pcm[w*512 .. w*512+576) (pcm starts with the 64 samples before the block), reflect-padded by 128;
-  //    the final 64 samples of the audio's last window are zero (SileroVADModel zeroes them in place)
-  for (int i = threadIdx.x; i < kTile * kPadded; i += kThreads) {
-    const int w = i / kPadded, j = i % kPadded;
-    int s = j - kPad;
-    s = s < 0 ? -s : (s >= kIn ? 2 * (kIn - 1) - s : s);
-    const int n = n0 + w;
-    const bool zero = n >= nb || (last_is_tail && n == nb - 1 && s >= kIn - kCtx);
-    A[i] = zero ? 0.f : pcm[(int64_t)n * kWin + s];
+  if (threadIdx.x < kTile) {
+    const int n = n0 + threadIdx.x;
+    int64_t at = -1;
+    int flags = 0;
+    if (n < nb) {
+      const VadSlice sl = slices[vad_find_slice(slices, n_slices, n)];
+      const int k = n - sl.w0;
+      at = sl.pcm0 + (int64_t)k * kWin;
+      flags = (sl.first && k == 0 ? 1 : 0) | (sl.last && k == sl.nb - 1 ? 2 : 0);
+    }
+    win_pcm[threadIdx.x] = at;
+    win_flags[threadIdx.x] = flags;
+  }
+  __syncthreads();
+  // 1. inputs: window k of a slice is pcm[pcm0 + k*512 .. + 576) (a slice's pcm starts with the 64 samples before it),
+  //    reflect-padded by 128; the context of a stream's first window is zero, and so are the final 64 samples of its last
+  //    window (SileroVADModel zeroes them in place)
+  static_assert(kTile % (kThreads / 32) == 0, "whole windows per warp");
+  for (int w = threadIdx.x >> 5; w < kTile; w += kThreads / 32) {  // a warp per window: its slice entry is read once
+    const int64_t at = win_pcm[w];
+    const int fl = win_flags[w];
+    for (int j = threadIdx.x & 31; j < kPadded; j += 32) {
+      int s = j - kPad;
+      s = s < 0 ? -s : (s >= kIn ? 2 * (kIn - 1) - s : s);
+      const bool zero = at < 0 || ((fl & 1) && s < kCtx) || ((fl & 2) && s >= kIn - kCtx);
+      A[w * kPadded + j] = zero ? 0.f : pcm[at + s];
+    }
   }
   __syncthreads();
   // 2. STFT magnitude: bin b of frames 1..4 (frame 0 is dropped) for half of the tile's windows per item
@@ -153,10 +186,17 @@ static __device__ __forceinline__ void cluster_sync() {
 // 128 columns (interleaved by float4 so the four quarters read h from different banks).  Warp v of CTA `rank` owns hidden
 // units j = 32 rank + 2 v + u.  Lane 16 u gathers the four gates of its unit, updates c (kept in its register) and h, stores
 // h to H and into the next h buffer of all four CTAs.
+// Cluster blockIdx.x / 4 runs slice blockIdx.x / 4 from its stream's h and c (zero when the slice starts the stream) and leaves
+// them there for the stream's next slice.
 __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kRecThreads, 1)
-    vad_recurrence_kernel(const float* __restrict__ w_hh, const float* __restrict__ gx, int nb, float* __restrict__ state_h,
-                          float* __restrict__ state_c, float* __restrict__ H) {
+    vad_recurrence_kernel(const float* __restrict__ w_hh, const VadSlice* __restrict__ slices, const float* __restrict__ gx,
+                          float* __restrict__ states, float* __restrict__ H) {
   __shared__ __align__(16) float hbuf[2][kHidden];
+  const VadSlice sl = slices[blockIdx.x / kCluster];
+  const int nb = sl.nb;
+  const bool first = sl.first;
+  float* __restrict__ state_h = states + (int64_t)sl.stream * 2 * kHidden;
+  float* __restrict__ state_c = state_h + kHidden;
   const int rank = (int)cluster_ctarank();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int u = lane >> 4, g = (lane >> 2) & 3, q = lane & 3;
@@ -166,15 +206,17 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kRecThreads, 
   float4 w[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) w[i] = __ldg(reinterpret_cast<const float4*>(w_hh + (size_t)row * kHidden) + 4 * i + q);
-  for (int i = threadIdx.x; i < kHidden; i += kRecThreads) hbuf[0][i] = state_h[i];
-  float c = owner ? state_c[j] : 0.f, h = 0.f;
+  for (int i = threadIdx.x; i < kHidden; i += kRecThreads) hbuf[0][i] = first ? 0.f : state_h[i];
+  float c = owner && !first ? state_c[j] : 0.f, h = 0.f;
   // Gx[n + 2] is loaded during step n and must have arrived when the registers rotate at the end of that step: the load
   // overlaps one whole step
-  float gx0 = nb > 0 ? __ldg(gx + row) : 0.f;
-  float gx1 = nb > 1 ? __ldg(gx + kGates + row) : 0.f;
+  const float* __restrict__ gx_row = gx + (int64_t)sl.w0 * kGates + row;  // this unit's gate row of the slice's first window
+  float* __restrict__ h_out = H + (int64_t)sl.w0 * kHidden + j;
+  float gx0 = nb > 0 ? __ldg(gx_row) : 0.f;
+  float gx1 = nb > 1 ? __ldg(gx_row + kGates) : 0.f;
   cluster_sync();  // every CTA of the cluster runs and holds h0 before anyone writes into its shared memory
   for (int n = 0; n < nb; ++n) {
-    const float gx2 = n + 2 < nb ? __ldg(gx + (int64_t)(n + 2) * kGates + row) : 0.f;
+    const float gx2 = n + 2 < nb ? __ldg(gx_row + (int64_t)(n + 2) * kGates) : 0.f;
     const float4* h4 = reinterpret_cast<const float4*>(hbuf[n & 1]);
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
 #pragma unroll
@@ -194,7 +236,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kRecThreads, 
     if (owner) {
       c = sigmoidf_(gf) * c + sigmoidf_(gi) * tanhf(gc);
       h = sigmoidf_(go) * tanhf(c);
-      H[(int64_t)n * kHidden + j] = h;
+      h_out[(int64_t)n * kHidden] = h;
       float* dst = &hbuf[(n + 1) & 1][j];
 #pragma unroll
       for (int r = 0; r < kCluster; ++r) st_cluster_f32(dst, r, h);
@@ -224,13 +266,14 @@ void vad_configure() {
   B2W_CUDA(cudaFuncSetAttribute(vad_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWindowSmem));
 }
 
-void vad_windows(const VadWeights& w, const float* pcm, int nb, bool last_is_tail, float* gx, cudaStream_t s) {
-  vad_window_kernel<<<ceil_div(nb, kTile), kThreads, kWindowSmem, s>>>(w, pcm, nb, last_is_tail ? 1 : 0, gx);
+void vad_windows(const VadWeights& w, const float* pcm, const VadSlice* slices, int n_slices, int nb, float* gx, cudaStream_t s) {
+  vad_window_kernel<<<ceil_div(nb, kTile), kThreads, kWindowSmem, s>>>(w, pcm, slices, n_slices, nb, gx);
   B2W_LAUNCHED();
 }
 
-void vad_recurrence(const float* w_hh, const float* gx, int nb, float* state_h, float* state_c, float* H, cudaStream_t s) {
-  vad_recurrence_kernel<<<kCluster, kRecThreads, 0, s>>>(w_hh, gx, nb, state_h, state_c, H);
+void vad_recurrence(const float* w_hh, const VadSlice* slices, int n_slices, const float* gx, float* states, float* H,
+                    cudaStream_t s) {
+  vad_recurrence_kernel<<<kCluster * n_slices, kRecThreads, 0, s>>>(w_hh, slices, gx, states, H);
   B2W_LAUNCHED();
 }
 

@@ -13,12 +13,24 @@ struct VadWeights {
   const float* b_gates = nullptr;  // [512]: b_ih + b_hh
 };
 
+// One stream's share of a launch: windows w0 .. w0 + nb - 1 of the launch's concatenated windows (nb >= 1, slices in window
+// order).  Its PCM sits at pcm + pcm0: the 64 samples before its first window, then its nb windows.
+struct VadSlice {
+  int64_t pcm0;
+  int32_t w0, nb;
+  int32_t stream;  // row of the per-stream LSTM state (h [128] then c [128]) carried between launches
+  int32_t first;   // the slice starts the stream: zero context, zero h and c
+  int32_t last;    // the slice ends the stream: the last window's final 64 samples count as zero
+  int32_t pad_;
+};
+
 void vad_configure();  // per-device kernel attributes
-// Gx[n][512] = W_ih x_n + b for the nb windows of a block.  pcm: 64 + 512 nb samples, the 64 before the block's first window
-// (zeros at the start of the audio) followed by the block; last_is_tail: the block's last window is the audio's last window.
-void vad_windows(const VadWeights& w, const float* pcm, int nb, bool last_is_tail, float* gx, cudaStream_t s);
-// The LSTM over nb steps in one launch, from and back to state_h / state_c [128]; H[n][128] receives every step's h.
-void vad_recurrence(const float* w_hh, const float* gx, int nb, float* state_h, float* state_c, float* H, cudaStream_t s);
+// Gx[n][512] = W_ih x_n + b for the nb windows of a launch (device table `slices`, n_slices entries).
+void vad_windows(const VadWeights& w, const float* pcm, const VadSlice* slices, int n_slices, int nb, float* gx, cudaStream_t s);
+// The LSTM over every slice in one launch, one 4-CTA cluster per slice, from and back to its stream's state
+// states[stream][256]; H[n][128] receives every window's h.
+void vad_recurrence(const float* w_hh, const VadSlice* slices, int n_slices, const float* gx, float* states, float* H,
+                    cudaStream_t s);
 // probs[n] = sigmoid(w . relu(H[n]) + b[0])
 void vad_decoder(const float* H, const float* w, const float* b, int nb, float* probs, cudaStream_t s);
 

@@ -146,7 +146,7 @@ ABI_SYMBOLS = (
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
     "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
-    "b2w_debug_step_logits", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_set_block", "b2w_vad_timing",
+    "b2w_debug_step_logits", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
 )
 
 
@@ -216,6 +216,8 @@ def load_library():
         lib.b2w_vad_destroy.argtypes = [C.c_void_p]
         lib.b2w_vad_destroy.restype = None
         lib.b2w_vad_probs.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        lib.b2w_vad_probs_multi.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.c_void_p,
+                                            C.c_int64]
         lib.b2w_vad_set_block.argtypes = [C.c_void_p, C.c_int64]
         lib.b2w_vad_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         if lib.b2w_abi_version() != 1:
@@ -734,8 +736,21 @@ class SileroVad:
         _check(self._lib.b2w_vad_probs(self._h, _ptr(x), x.shape[0], _ptr(out), out.shape[0]))
         return out
 
+    def probs_many(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """``probs`` of several independent recordings in one sequence of launches (``b2w_vad_probs_multi``); each result is
+        bit-identical to ``probs`` of that recording alone."""
+        xs = [np.ascontiguousarray(p, dtype=np.float32) for p in pcms]
+        if not xs:
+            return []
+        ptrs = (C.c_void_p * len(xs))(*[x.ctypes.data for x in xs])
+        lens = (C.c_int64 * len(xs))(*[x.shape[0] for x in xs])
+        out = np.empty(max(sum(x.shape[0] // 512 for x in xs), 1), np.float32)
+        _check(self._lib.b2w_vad_probs_multi(self._h, ptrs, lens, len(xs), _ptr(out), out.shape[0]))
+        bounds = np.cumsum([0] + [x.shape[0] // 512 for x in xs])
+        return [out[lo:hi].copy() for lo, hi in zip(bounds[:-1], bounds[1:])]
+
     def timing(self) -> Dict[str, float]:
-        """Device milliseconds of the last ``probs`` call per kernel."""
+        """Device milliseconds of the last ``probs`` or ``probs_many`` call per kernel."""
         ms = (C.c_double * 3)()
         _check(self._lib.b2w_vad_timing(self._h, ms))
         return dict(zip(("window", "recurrence", "decoder"), ms))

@@ -18,7 +18,7 @@ import zlib
 from dataclasses import asdict, dataclass
 from inspect import signature
 from math import ceil
-from typing import BinaryIO, Iterable, Iterator, List, Optional, Tuple, Union
+from typing import BinaryIO, Iterable, Iterator, List, Optional, Sequence, Tuple, Union
 from warnings import warn
 
 import numpy as np
@@ -29,7 +29,7 @@ from .config import MODEL_DIMS
 from .feature_extractor import FeatureExtractor
 from .tokenizer import _LANGUAGE_CODES, Tokenizer
 from .utils import download_model, format_timestamp, get_end, get_logger
-from .vad import SpeechTimestampsMap, VadOptions, collect_chunks, get_speech_timestamps
+from .vad import SpeechTimestampsMap, VadOptions, collect_chunks, get_speech_timestamps, get_speech_timestamps_many
 
 _DEFAULT_TEMPERATURES = [0.0, 0.2, 0.4, 0.6, 0.8, 1.0]
 _PREPEND_PUNCT = "\"'“¿([{-"
@@ -201,6 +201,45 @@ def _check_max_length(prompt_len: int, max_new_tokens: Optional[int], limit: int
     return total
 
 
+@dataclass
+class _FilePlan:
+    """One recording's share of a batched transcription: its chunks, their metadata, and what finishes its segments."""
+    chunks: List[np.ndarray]
+    metadata: List[dict]
+    spans: List[dict]          # VAD spans, the whole file, or the user's clips (in samples)
+    from_user: bool            # the chunks are user clips: segment times are not mapped back
+    duration: float = 0.0
+    duration_after_vad: float = 0.0
+    tokenizer: Optional[Tokenizer] = None
+    options: Optional[TranscriptionOptions] = None
+    info: Optional[TranscriptionInfo] = None
+
+
+class _LanguageVote:
+    """``WhisperModel.detect_language``'s rule over successive 30 s windows of one recording: the first window whose top
+    language is above the threshold decides, otherwise the language found in most windows, with its best probability."""
+
+    def __init__(self, threshold: float):
+        self.threshold = threshold
+        self.votes: dict = {}
+        self.decided = None
+        self.all_language_probs = None
+
+    def add(self, ranked: List[Tuple[str, float]]) -> None:
+        self.all_language_probs = [(tok[2:-2], p) for tok, p in ranked]
+        language, probability = self.all_language_probs[0]
+        if probability > self.threshold:
+            self.decided = (language, probability, self.all_language_probs)
+        else:
+            self.votes.setdefault(language, []).append(probability)
+
+    def result(self) -> Tuple[str, float, List[Tuple[str, float]]]:
+        if self.decided is not None:
+            return self.decided
+        language = max(self.votes, key=lambda k: len(self.votes[k]))
+        return language, max(self.votes[language]), self.all_language_probs
+
+
 # --------------------------------------------------------------------------------------------------
 # batched pipeline (transcribe.py:111-617)
 # --------------------------------------------------------------------------------------------------
@@ -210,45 +249,69 @@ class BatchedInferencePipeline:
         self.last_speech_timestamp = 0.0
 
     # -- one batch: encode + one generate call + timestamp splitting ---------------------------------
-    def forward(self, features, tokenizer, chunks_metadata, options):
-        encoder_output, outputs = self.generate_segment_batched(features, tokenizer, options)
+    def forward(self, features, tokenizer, chunks_metadata, options, last_speech: Optional[dict] = None):
+        """`tokenizer`: one Tokenizer, or one per chunk when the chunks come from several recordings (their metadata carry
+        the recording's index as "file").  `last_speech`: per recording, the end of its last word so far (word timestamps),
+        updated in place; by default the pipeline's `last_speech_timestamp` runs through every chunk."""
+        tokenizers = list(tokenizer) if isinstance(tokenizer, (list, tuple)) else [tokenizer] * len(chunks_metadata)
+        encoder_output, outputs = self.generate_segment_batched(features, tokenizers, options)
         model = self.model
         batch_results, frame_counts = [], []
-        for meta, out in zip(chunks_metadata, outputs):
+        for meta, out, tok in zip(chunks_metadata, outputs, tokenizers):
             n_frames = int(ceil(meta["duration"]) * model.frames_per_second)
             frame_counts.append(n_frames)
             pieces, _, _ = model._split_segments_by_timestamps(
-                tokenizer=tokenizer, tokens=out["tokens"], time_offset=meta["offset"], segment_size=n_frames,
+                tokenizer=tok, tokens=out["tokens"], time_offset=meta["offset"], segment_size=n_frames,
                 segment_duration=meta["duration"], seek=0)
             rows = []
             for piece in pieces:
-                text = tokenizer.decode(piece["tokens"])
+                text = tok.decode(piece["tokens"])
                 rows.append(dict(
                     text=text, avg_logprob=out["avg_logprob"], no_speech_prob=out["no_speech_prob"], tokens=piece["tokens"],
                     start=piece["start"], end=piece["end"], compression_ratio=get_compression_ratio(text),
                     seek=int(meta["offset"] * model.frames_per_second)))
             batch_results.append(rows)
         if options.word_timestamps:
-            self.last_speech_timestamp = model.add_word_timestamps(
-                batch_results, tokenizer, encoder_output, frame_counts, options.prepend_punctuations,
-                options.append_punctuations, self.last_speech_timestamp)
+            ends = last_speech if last_speech is not None else {0: self.last_speech_timestamp}
+            # one align call per distinct start sequence (it holds the language token), items of other languages empty
+            aligned = [None] * len(batch_results)
+            starts = list(dict.fromkeys(tuple(t.sot_sequence) for t in tokenizers))
+            for start in starts:
+                mine = [tuple(t.sot_sequence) == start for t in tokenizers]
+                text_tokens = [model.text_tokens(rows, tok.eot) if m else [] for rows, tok, m in zip(batch_results, tokenizers, mine)]
+                for i, r in enumerate(model.model.align(encoder_output, list(start), text_tokens, frame_counts, median_filter_width=7)):
+                    if mine[i]:
+                        aligned[i] = r
+            # words per recording, in chunk order, each with its own tokenizer and running end of speech
+            files = [meta.get("file", 0) for meta in chunks_metadata]
+            for f in dict.fromkeys(files):
+                idx = [i for i, g in enumerate(files) if g == f]
+                ends[f] = model.assemble_words(
+                    [batch_results[i] for i in idx], tokenizers[idx[0]], [aligned[i] for i in idx], options.prepend_punctuations,
+                    options.append_punctuations, ends.get(f, 0.0))
+            if last_speech is None:
+                self.last_speech_timestamp = ends[0]
         return batch_results
 
-    def generate_segment_batched(self, features, tokenizer: Tokenizer, options: TranscriptionOptions):
+    def generate_segment_batched(self, features, tokenizer, options: TranscriptionOptions):
         """`features` is either the stacked float32 array [n, n_mels, 3000] (reference contract) or an encoder
-        output already produced by the fused audio path."""
+        output already produced by the fused audio path.  `tokenizer`: one Tokenizer, or one per chunk (prompts that differ
+        only in their language token)."""
         model = self.model
         n = features.shape[0]
-        history = tokenizer.encode(options.initial_prompt) if options.initial_prompt is not None else []
-        prompt = model.get_prompt(tokenizer, previous_tokens=history, without_timestamps=options.without_timestamps,
-                                  hotwords=options.hotwords)
-        max_length = _check_max_length(len(prompt), options.max_new_tokens, model.max_length)
+        tokenizers = list(tokenizer) if isinstance(tokenizer, (list, tuple)) else [tokenizer] * n
+        made = {}
+        for tok in tokenizers:
+            if id(tok) not in made:
+                history = tok.encode(options.initial_prompt) if options.initial_prompt is not None else []
+                made[id(tok)] = model.get_prompt(tok, previous_tokens=history, without_timestamps=options.without_timestamps,
+                                                 hotwords=options.hotwords)
+        prompts = [list(made[id(tok)]) for tok in tokenizers]
+        max_length = _check_max_length(len(prompts[0]), options.max_new_tokens, model.max_length)
         encoder_output = features if isinstance(features, engine.StorageView) else model.encode(features)
-        prompts = [list(prompt) for _ in range(n)]
         if options.multilingual:
-            where = prompt.index(tokenizer.language)
-            for row, langs in zip(prompts, model.model.detect_language(encoder_output)):
-                row[where] = tokenizer.tokenizer.token_to_id(langs[0][0])
+            for row, tok, langs in zip(prompts, tokenizers, model.model.detect_language(encoder_output)):
+                row[row.index(tok.language)] = tok.tokenizer.token_to_id(langs[0][0])
         results = model.model.generate(
             encoder_output, prompts, beam_size=options.beam_size, patience=options.patience,
             length_penalty=options.length_penalty, max_length=max_length, suppress_blank=options.suppress_blank,
@@ -305,108 +368,184 @@ class BatchedInferencePipeline:
         engine call.  Arguments, defaults and the ignored ones (compression/log-prob/no-speech thresholds,
         condition_on_previous_text, prefix, max_initial_timestamp, hallucination_silence_threshold) follow the
         reference (transcribe.py:254-375).  Returns (lazy segment generator, TranscriptionInfo)."""
+        kw = {k: v for k, v in locals().items() if k not in ("self", "audio", "clip_timestamps")}
+        plan = self._prepare([audio], [clip_timestamps], kw)[0]
+        segments = (seg for _, seg in self._batched_segments_generator(
+            plan.chunks, [plan.tokenizer] * len(plan.chunks), plan.metadata, batch_size, plan.options, log_progress))
+        if not plan.from_user:
+            segments = restore_speech_timestamps(segments, plan.spans, self.model.feature_extractor.sampling_rate)
+        return segments, plan.info
+
+    def transcribe_many(self, audios: Sequence[Union[str, BinaryIO, np.ndarray]],
+                        clip_timestamps: Optional[Sequence[Optional[List[dict]]]] = None,
+                        **kwargs) -> List[Tuple[List[Segment], TranscriptionInfo]]:
+        """Transcribes several recordings in one pass: the chunks of all of them, in file order then chunk order, share
+        decode batches of `batch_size` chunks, and the VAD of every recording that needs it runs in one multi-stream GPU call.
+        `clip_timestamps`: None, or one list of {"start", "end"} (or None) per recording; every other keyword argument is
+        `transcribe()`'s, with its default.
+
+        Returns one (segments, TranscriptionInfo) per recording, in input order, equal to `transcribe(audios[i], ...)` apart
+        from the engine's own dependence on which chunks share a batch.  The segments are lists, computed before this
+        returns: a batch holds chunks of several recordings, so a per-recording generator would have to buffer anyway."""
+        params = signature(self.transcribe).parameters
+        unknown = sorted(set(kwargs) - set(params) - {"audio", "clip_timestamps"})
+        if unknown:
+            raise TypeError(f"transcribe_many() got unexpected keyword arguments: {', '.join(unknown)}")
+        kw = {k: p.default for k, p in params.items() if k not in ("audio", "clip_timestamps")}
+        kw.update(kwargs)
+        audios = list(audios)
+        clips = [None] * len(audios) if clip_timestamps is None else list(clip_timestamps)
+        if len(clips) != len(audios):
+            raise ValueError("clip_timestamps must hold one entry (a list of clips, or None) per recording")
+        plans = self._prepare(audios, clips, kw)
+        if not plans:
+            return []
+        for p in plans[1:]:
+            assert p.options.suppress_tokens == plans[0].options.suppress_tokens, "suppress_tokens differ between recordings"
+        chunks, metadata, tokenizers = [], [], []
+        for fi, p in enumerate(plans):
+            chunks += p.chunks
+            metadata += [dict(m, file=fi) for m in p.metadata]
+            tokenizers += [p.tokenizer] * len(p.chunks)
+        segments = [[] for _ in plans]
+        for fi, seg in self._batched_segments_generator(chunks, tokenizers, metadata, kw["batch_size"], plans[0].options,
+                                                        kw["log_progress"], last_speech={}):
+            segments[fi].append(seg)
+        sr = self.model.feature_extractor.sampling_rate
+        return [(segs if p.from_user else list(restore_speech_timestamps(segs, p.spans, sr)), p.info)
+                for p, segs in zip(plans, segments)]
+
+    def _prepare(self, audios, clips, kw) -> List[_FilePlan]:
+        """Per recording: decode it, carve it into <= chunk_length pieces (the user's clips, VAD spans, or the whole file when
+        it is shorter than chunk_length), then its language, tokenizer, options and TranscriptionInfo.  The VAD of every
+        recording without clips runs in one call, and language detection in one encode + detect_language per round and
+        batch_size recordings."""
         model = self.model
         sr = model.feature_extractor.sampling_rate
+        multilingual = kw["multilingual"]
         if multilingual and not model.model.is_multilingual:
             model.logger.warning("The current model is English-only but the multilingual parameter is set to"
                                  "True; setting to False instead.")
             multilingual = False
-        if not isinstance(audio, np.ndarray):
-            audio = decode_audio(audio, sampling_rate=sr)
-        duration = audio.shape[0] / sr
-        model.logger.info("Processing audio with duration %s", format_timestamp(duration))
-        chunk_length = chunk_length or model.feature_extractor.chunk_length
+        chunk_length = kw["chunk_length"] or model.feature_extractor.chunk_length
+        pcm = []
+        for audio in audios:
+            if not isinstance(audio, np.ndarray):
+                audio = decode_audio(audio, sampling_rate=sr)
+            model.logger.info("Processing audio with duration %s", format_timestamp(audio.shape[0] / sr))
+            pcm.append(audio)
 
-        # ---- carve the audio into <= chunk_length pieces -------------------------------------------------
-        if clip_timestamps:
-            from_user = True
-            clip_timestamps = [{k: int(v * sr) for k, v in clip.items()} for clip in clip_timestamps]
-            audio_chunks, chunks_metadata = [], []
-            for i, clip in enumerate(clip_timestamps):
-                audio_chunks.append(audio[clip["start"] : clip["end"]])
-                seconds = (clip["end"] - clip["start"]) / sr
-                if seconds > 30:
-                    model.logger.warning("Segment %d is longer than 30 seconds, only the first 30 seconds will be transcribed", i)
-                chunks_metadata.append({"offset": clip["start"] / sr, "duration": seconds, "segments": [clip]})
-        else:
-            from_user = False
-            if vad_filter:
-                if vad_parameters is None:
-                    vad_parameters = VadOptions(max_speech_duration_s=chunk_length, min_silence_duration_ms=160)
-                elif isinstance(vad_parameters, dict):
-                    vad_parameters = VadOptions(**{**{k: v for k, v in vad_parameters.items() if k != "max_speech_duration_s"},
-                                                   "max_speech_duration_s": chunk_length})
-                clip_timestamps = get_speech_timestamps(audio, vad_parameters, device_index=model.model.device_index[0])
-            elif duration < chunk_length:
-                clip_timestamps = [{"start": 0, "end": audio.shape[0]}]
-            else:
-                raise RuntimeError("No clip timestamps found. Set 'vad_filter' to True or provide 'clip_timestamps'.")
-            audio_chunks, chunks_metadata = collect_chunks(audio, clip_timestamps, max_duration=chunk_length)
+        vad_parameters = kw["vad_parameters"]
+        vad_options = [vad_parameters] * len(pcm)
+        vad_files = [i for i, c in enumerate(clips) if not c] if kw["vad_filter"] else []
+        speech = {}
+        if vad_files:
+            if vad_parameters is None:
+                vad_parameters = VadOptions(max_speech_duration_s=chunk_length, min_silence_duration_ms=160)
+            elif isinstance(vad_parameters, dict):
+                vad_parameters = VadOptions(**{**{k: v for k, v in vad_parameters.items() if k != "max_speech_duration_s"},
+                                               "max_speech_duration_s": chunk_length})
+            spans = get_speech_timestamps_many([pcm[i] for i in vad_files], vad_parameters, device_index=model.model.device_index[0])
+            speech = dict(zip(vad_files, spans))
+            for i in vad_files:
+                vad_options[i] = vad_parameters
 
-        duration_after_vad = sum(c["end"] - c["start"] for c in clip_timestamps) / sr
-        model.logger.info("VAD filter removed %s of audio", format_timestamp(duration - duration_after_vad))
-        if not duration_after_vad:
-            audio_chunks, chunks_metadata = [], []
-        # (a chunk longer than 30 s — only possible with user-supplied clips — is not cut here: like the reference, its log-mel is computed
-        #  over the whole clip and the FEATURES are trimmed to 3000 frames, see _batched_segments_generator)
+        plans = []
+        for i, audio in enumerate(pcm):
+            plan = self._carve(audio, clips[i], speech.get(i), chunk_length)
+            plan.duration = audio.shape[0] / sr
+            plan.duration_after_vad = sum(c["end"] - c["start"] for c in plan.spans) / sr
+            model.logger.info("VAD filter removed %s of audio", format_timestamp(plan.duration - plan.duration_after_vad))
+            if not plan.duration_after_vad:
+                plan.chunks, plan.metadata = [], []
+            plans.append(plan)
 
-        # ---- language ---------------------------------------------------------------------------------------
-        all_language_probs = None
-        if language is None:
-            if not model.model.is_multilingual:
-                language, language_probability = "en", 1
-            else:
-                # the reference concatenates the features of ALL chunks and detect_language reads the first
-                # `language_detection_segments` windows of 3000 frames (transcribe.py:478-489): short leading chunks are followed by the
-                # next chunks' frames inside a window.  Only the chunks that reach into those windows are computed here.
-                feats, need = [], max(1, language_detection_segments) * model.feature_extractor.nb_max_frames
-                for c in audio_chunks:
+        language, segments_ = kw["language"], kw["language_detection_segments"]
+        if language is None and model.model.is_multilingual:
+            # the reference concatenates the features of ALL chunks and detect_language reads the first
+            # `language_detection_segments` windows of 3000 frames (transcribe.py:478-489): short leading chunks are followed by the
+            # next chunks' frames inside a window.  Only the chunks that reach into those windows are computed here.
+            need = max(1, segments_) * model.feature_extractor.nb_max_frames
+            features = []
+            for plan in plans:
+                feats = []
+                for c in plan.chunks:
                     if sum(f.shape[-1] for f in feats) >= need:
                         break
                     feats.append(model.feature_extractor(c)[..., :-1])
                 feats.append(np.full((model.model.n_mels, 1), -1.5, dtype="float32"))  # keeps empty audio well-formed
-                language, language_probability, all_language_probs = model.detect_language(
-                    features=np.concatenate(feats, axis=1), language_detection_segments=language_detection_segments,
-                    language_detection_threshold=language_detection_threshold)
-                model.logger.info("Detected language '%s' with probability %.2f", language, language_probability)
+                features.append(np.concatenate(feats, axis=1))
+            languages = model.detect_languages(features, segments_, kw["language_detection_threshold"], kw["batch_size"])
+            for lang, prob, _ in languages:
+                model.logger.info("Detected language '%s' with probability %.2f", lang, prob)
         else:
-            if not model.model.is_multilingual and language != "en":
+            if language is None:
+                language = "en"
+            elif not model.model.is_multilingual and language != "en":
                 model.logger.warning("The current model is English-only but the language parameter is set to '%s'; "
                                      "using 'en' instead." % language)
                 language = "en"
-            language_probability = 1
+            languages = [(language, 1, None)] * len(plans)
 
-        tokenizer = Tokenizer(model.hf_tokenizer, model.model.is_multilingual, task=task, language=language)
-        options = TranscriptionOptions(
-            beam_size=beam_size, best_of=best_of, patience=patience, length_penalty=length_penalty,
-            repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
-            log_prob_threshold=log_prob_threshold, no_speech_threshold=no_speech_threshold,
-            compression_ratio_threshold=compression_ratio_threshold, temperatures=_as_temperature_list(temperature)[:1],
-            initial_prompt=initial_prompt, prefix=prefix, suppress_blank=suppress_blank,
-            suppress_tokens=get_suppressed_tokens(tokenizer, suppress_tokens) if suppress_tokens else suppress_tokens,
-            prepend_punctuations=prepend_punctuations, append_punctuations=append_punctuations,
-            max_new_tokens=max_new_tokens, hotwords=hotwords, word_timestamps=word_timestamps,
-            hallucination_silence_threshold=None, condition_on_previous_text=False, clip_timestamps=clip_timestamps,
-            prompt_reset_on_temperature=0.5, multilingual=multilingual, without_timestamps=without_timestamps,
-            max_initial_timestamp=0.0)
-        info = TranscriptionInfo(
-            language=language, language_probability=language_probability, duration=duration,
-            duration_after_vad=duration_after_vad, transcription_options=options, vad_options=vad_parameters,
-            all_language_probs=all_language_probs)
-        segments = self._batched_segments_generator(audio_chunks, tokenizer, chunks_metadata, batch_size, options, log_progress)
-        if not from_user:
-            segments = restore_speech_timestamps(segments, clip_timestamps, sr)
-        return segments, info
+        for plan, (lang, prob, all_probs), vad_opts in zip(plans, languages, vad_options):
+            tokenizer = Tokenizer(model.hf_tokenizer, model.model.is_multilingual, task=kw["task"], language=lang)
+            suppress_tokens = kw["suppress_tokens"]
+            options = TranscriptionOptions(
+                beam_size=kw["beam_size"], best_of=kw["best_of"], patience=kw["patience"], length_penalty=kw["length_penalty"],
+                repetition_penalty=kw["repetition_penalty"], no_repeat_ngram_size=kw["no_repeat_ngram_size"],
+                log_prob_threshold=kw["log_prob_threshold"], no_speech_threshold=kw["no_speech_threshold"],
+                compression_ratio_threshold=kw["compression_ratio_threshold"],
+                temperatures=_as_temperature_list(kw["temperature"])[:1], initial_prompt=kw["initial_prompt"],
+                prefix=kw["prefix"], suppress_blank=kw["suppress_blank"],
+                suppress_tokens=get_suppressed_tokens(tokenizer, suppress_tokens) if suppress_tokens else suppress_tokens,
+                prepend_punctuations=kw["prepend_punctuations"], append_punctuations=kw["append_punctuations"],
+                max_new_tokens=kw["max_new_tokens"], hotwords=kw["hotwords"], word_timestamps=kw["word_timestamps"],
+                hallucination_silence_threshold=None, condition_on_previous_text=False, clip_timestamps=plan.spans,
+                prompt_reset_on_temperature=0.5, multilingual=multilingual, without_timestamps=kw["without_timestamps"],
+                max_initial_timestamp=0.0)
+            plan.tokenizer, plan.options = tokenizer, options
+            plan.info = TranscriptionInfo(
+                language=lang, language_probability=prob, duration=plan.duration, duration_after_vad=plan.duration_after_vad,
+                transcription_options=options, vad_options=vad_opts, all_language_probs=all_probs)
+        return plans
 
-    def _batched_segments_generator(self, features, tokenizer, chunks_metadata, batch_size, options, log_progress):
+    def _carve(self, audio: np.ndarray, clips: Optional[List[dict]], speech: Optional[List[dict]], chunk_length) -> _FilePlan:
+        """The chunks of one recording: its clips (seconds) when given, else its VAD spans `speech` (samples) when VAD ran,
+        else the whole recording if it is shorter than chunk_length."""
+        model = self.model
+        sr = model.feature_extractor.sampling_rate
+        if clips:
+            spans = [{k: int(v * sr) for k, v in clip.items()} for clip in clips]
+            chunks, metadata = [], []
+            for i, clip in enumerate(spans):
+                chunks.append(audio[clip["start"] : clip["end"]])
+                seconds = (clip["end"] - clip["start"]) / sr
+                if seconds > 30:
+                    model.logger.warning("Segment %d is longer than 30 seconds, only the first 30 seconds will be transcribed", i)
+                metadata.append({"offset": clip["start"] / sr, "duration": seconds, "segments": [clip]})
+            # (a chunk longer than 30 s is not cut here: like the reference, its log-mel is computed over the whole clip and the
+            #  FEATURES are trimmed to 3000 frames, see _batched_segments_generator)
+            return _FilePlan(chunks, metadata, spans, from_user=True)
+        if speech is not None:
+            spans = speech
+        elif audio.shape[0] / sr < chunk_length:
+            spans = [{"start": 0, "end": audio.shape[0]}]
+        else:
+            raise RuntimeError("No clip timestamps found. Set 'vad_filter' to True or provide 'clip_timestamps'.")
+        chunks, metadata = collect_chunks(audio, spans, max_duration=chunk_length)
+        return _FilePlan(chunks, metadata, spans, from_user=False)
+
+    def _batched_segments_generator(self, features, tokenizers, chunks_metadata, batch_size, options, log_progress,
+                                    last_speech: Optional[dict] = None):
         """`features`: list of PCM chunks (fused audio->mel->encoder path, the default here) or the reference's
-        stacked feature array [n, n_mels, 3000]."""
+        stacked feature array [n, n_mels, 3000]; `tokenizers`: one per chunk.  Yields (recording index, Segment) with
+        segment ids counted per recording (the metadata's "file", 0 when absent)."""
         from tqdm import tqdm
 
         fused = isinstance(features, list)
         total = len(features)
         bar = tqdm(total=total, disable=not log_progress, position=0)
-        seg_id = 0
+        seg_ids = {}
         for lo in range(0, total, batch_size):
             block = features[lo : lo + batch_size]
             if fused:
@@ -417,11 +556,13 @@ class BatchedInferencePipeline:
                     block = self.model.encode(np.stack([pad_or_trim(fe(c)[..., :-1]) for c in block]))
                 else:
                     block = self.model.model.encode_audio(block)
-            for rows in self.forward(block, tokenizer, chunks_metadata[lo : lo + batch_size], options):
+            metas = chunks_metadata[lo : lo + batch_size]
+            for meta, rows in zip(metas, self.forward(block, tokenizers[lo : lo + batch_size], metas, options, last_speech)):
+                f = meta.get("file", 0)
                 for row in rows:
-                    seg_id += 1
-                    yield Segment(
-                        seek=row["seek"], id=seg_id, text=row["text"], start=round(row["start"], 3), end=round(row["end"], 3),
+                    seg_ids[f] = seg_ids.get(f, 0) + 1
+                    yield f, Segment(
+                        seek=row["seek"], id=seg_ids[f], text=row["text"], start=round(row["start"], 3), end=round(row["end"], 3),
                         words=[Word(**w) for w in row["words"]] if options.word_timestamps else None, tokens=row["tokens"],
                         avg_logprob=row["avg_logprob"], no_speech_prob=row["no_speech_prob"],
                         compression_ratio=row["compression_ratio"], temperature=options.temperatures[0])
@@ -880,9 +1021,23 @@ class WhisperModel:
                             prepend_punctuations: str, append_punctuations: str, last_speech_timestamp: float) -> float:
         if len(segments) == 0:
             return last_speech_timestamp
+        text_tokens = [self.text_tokens(seg, tokenizer.eot) for seg in segments]
+        results = self.model.align(encoder_output, tokenizer.sot_sequence, text_tokens, num_frames, median_filter_width=7)
+        return self.assemble_words(segments, tokenizer, results, prepend_punctuations, append_punctuations, last_speech_timestamp)
+
+    @staticmethod
+    def text_tokens(segment: List[dict], eot: int) -> List[int]:
+        """The text tokens of one decoded window's sub-segments, as the alignment reads them."""
+        return [t for sub in segment for t in sub["tokens"] if t < eot]
+
+    def assemble_words(self, segments: List[dict], tokenizer: Tokenizer, align_results, prepend_punctuations: str,
+                       append_punctuations: str, last_speech_timestamp: float) -> float:
+        """Fills each sub-segment's "words" from the engine's alignment of its window (`align_results`, one per window, in
+        order), splitting words as `tokenizer`'s language does; `last_speech_timestamp` runs through the windows in order and
+        its final value is returned."""
         per_segment_tokens = [[[t for t in sub["tokens"] if t < tokenizer.eot] for sub in seg] for seg in segments]
         text_tokens = [list(itertools.chain.from_iterable(parts)) for parts in per_segment_tokens]
-        alignments = self.find_alignment(tokenizer, text_tokens, encoder_output, num_frames)
+        alignments = self._words_from_alignment(tokenizer, text_tokens, align_results)
         limits = []
         for alignment in alignments:
             spans = np.array([w["end"] - w["start"] for w in alignment])
@@ -939,6 +1094,9 @@ class WhisperModel:
             return []
         results = self.model.align(encoder_output, tokenizer.sot_sequence, text_tokens, num_frames,
                                    median_filter_width=median_filter_width)
+        return self._words_from_alignment(tokenizer, text_tokens, results)
+
+    def _words_from_alignment(self, tokenizer: Tokenizer, text_tokens, results) -> List[List[dict]]:
         out = []
         for result, toks in zip(results, text_tokens):
             words, word_tokens = tokenizer.split_to_word_tokens(toks + [tokenizer.eot])
@@ -973,16 +1131,28 @@ class WhisperModel:
                 pieces, _ = collect_chunks(audio, spans)
                 audio = np.concatenate(pieces, axis=0)
             features = fe(audio[: language_detection_segments * fe.n_samples])
-        features = features[..., : language_detection_segments * fe.nb_max_frames]
-        votes = {}
-        language = language_probability = all_language_probs = None
-        for lo in range(0, features.shape[-1], fe.nb_max_frames):
-            enc = self.encode(pad_or_trim(features[..., lo : lo + fe.nb_max_frames]))
-            ranked = self.model.detect_language(enc)[0]
-            all_language_probs = [(tok[2:-2], p) for tok, p in ranked]
-            language, language_probability = all_language_probs[0]
-            if language_probability > language_detection_threshold:
-                return language, language_probability, all_language_probs
-            votes.setdefault(language, []).append(language_probability)
-        language = max(votes, key=lambda k: len(votes[k]))
-        return language, max(votes[language]), all_language_probs
+        return self.detect_languages([features], language_detection_segments, language_detection_threshold)[0]
+
+    def detect_languages(self, features: List[np.ndarray], language_detection_segments: int = 1,
+                         language_detection_threshold: float = 0.5,
+                         batch_size: Optional[int] = None) -> List[Tuple[str, float, List[Tuple[str, float]]]]:
+        """``detect_language(features=f)`` for each recording's features f: round r encodes window r of every recording
+        still undecided and runs detect_language over them, `batch_size` windows per call (all of them when None), so the
+        encoder's memory stays bounded however many recordings there are."""
+        fe = self.feature_extractor
+        windows = []
+        for f in features:
+            f = f[..., : language_detection_segments * fe.nb_max_frames]
+            windows.append([pad_or_trim(f[..., lo : lo + fe.nb_max_frames]) for lo in range(0, f.shape[-1], fe.nb_max_frames)])
+        votes = [_LanguageVote(language_detection_threshold) for _ in features]
+        for r in range(max(map(len, windows), default=0)):
+            live = [i for i, w in enumerate(windows) if r < len(w) and votes[i].decided is None]
+            if not live:
+                break
+            step = batch_size or len(live)
+            for lo in range(0, len(live), step):
+                part = live[lo : lo + step]
+                enc = self.encode(np.stack([windows[i][r] for i in part]))
+                for i, ranked in zip(part, self.model.detect_language(enc)):
+                    votes[i].add(ranked)
+        return [v.result() for v in votes]

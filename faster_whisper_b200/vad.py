@@ -15,7 +15,7 @@ from __future__ import annotations
 import bisect
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -112,6 +112,12 @@ class SileroGpuVAD:
         assert num_samples == _WINDOW and context == 64, "the network takes 512-sample windows after 64 context samples"
         return self.model.probs(audio)
 
+    def many(self, audios: Sequence[np.ndarray], num_samples: int = _WINDOW, context: int = 64) -> List[np.ndarray]:
+        """``self(audio)`` for each of several padded recordings, all of them in one sequence of GPU launches."""
+        assert all(a.ndim == 1 and a.shape[0] % num_samples == 0 for a in audios)
+        assert num_samples == _WINDOW and context == 64, "the network takes 512-sample windows after 64 context samples"
+        return self.model.probs_many(audios)
+
 
 class _Segmenter:
     """Hysteresis over per-window speech probabilities (``vad.py:86-160``): speech starts at the first window >= threshold,
@@ -188,9 +194,27 @@ def get_speech_timestamps(audio: np.ndarray, vad_options: Optional[VadOptions] =
     """Speech spans ``[{"start": sample, "end": sample}, ...]`` (``vad.py:44-183``); ``device_index``: the GPU of the default
     Silero model when it runs on the GPU."""
     o = vad_options if vad_options is not None else VadOptions(**kwargs)
-    n = len(audio)
+    return _spans(audio, get_vad_model(device_index)(_padded(audio)), o, sampling_rate)
+
+
+def get_speech_timestamps_many(audios: Sequence[np.ndarray], vad_options: Optional[VadOptions] = None,
+                               sampling_rate: int = 16000, device_index: int = 0, **kwargs) -> List[List[dict]]:
+    """``get_speech_timestamps`` of every recording: the default GPU model runs all of them in one multi-stream call
+    (``SileroGpuVAD.many``); onnxruntime or a model installed by ``set_vad_model`` runs them one after another."""
+    o = vad_options if vad_options is not None else VadOptions(**kwargs)
     model = get_vad_model(device_index)
-    probs = model(np.pad(audio, (0, _WINDOW - audio.shape[0] % _WINDOW)))
+    padded = [_padded(a) for a in audios]
+    probs = model.many(padded) if hasattr(model, "many") else [model(a) for a in padded]
+    return [_spans(a, p, o, sampling_rate) for a, p in zip(audios, probs)]
+
+
+def _padded(audio: np.ndarray) -> np.ndarray:
+    return np.pad(audio, (0, _WINDOW - audio.shape[0] % _WINDOW))
+
+
+def _spans(audio: np.ndarray, probs: np.ndarray, o: VadOptions, sampling_rate: int) -> List[dict]:
+    """The segmenter over one recording's probabilities, then the span padding."""
+    n = len(audio)
     seg = _Segmenter(o, sampling_rate)
     for i, p in enumerate(probs):
         seg.feed(i, p)

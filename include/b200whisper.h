@@ -169,10 +169,19 @@ void b2w_vad_destroy(b2w_vad* vad);
  * last window's own final 64 samples count as zero.  The LSTM state starts at zero; the audio runs through in blocks of windows
  * (b2w_vad_set_block) with the state carried on the device, and the result does not depend on the block size. */
 int b2w_vad_probs(b2w_vad* vad, const float* pcm, int64_t n_samples, float* probs_out, int64_t capacity);
-/* Windows per block (default 32768, about 17.5 min of audio).  The block buffers take 4.6 KB of device memory per window (PCM,
- * LSTM inputs, hidden states, probabilities): 151 MB at the default. */
+/* b2w_vad_probs for n_streams independent recordings in one sequence of launches: stream i is pcm[i][n_samples[i]] (each a
+ * positive multiple of 512), and its probabilities follow those of stream i - 1 in probs_out (capacity in floats, at least the
+ * total number of windows).  Each launch runs one 4-CTA LSTM cluster per stream that still has windows, with that stream's state
+ * carried on the device, so every stream's probabilities are bit-identical to b2w_vad_probs on that stream alone, whatever
+ * the streams, their lengths and the block size.  Every argument is checked before any device work. */
+int b2w_vad_probs_multi(b2w_vad* vad, const float* const* pcm, const int64_t* n_samples, int32_t n_streams, float* probs_out,
+                        int64_t capacity);
+/* Windows per block (default 32768, about 17.5 min of audio), summed over the streams of a launch and split evenly over the
+ * streams that still have windows.  The block buffers take 4.6 KB of device memory per window (PCM, LSTM inputs, hidden
+ * states, probabilities): 151 MB at the default; each stream adds 1.3 KB (its LSTM state and the context before its slice). */
 int b2w_vad_set_block(b2w_vad* vad, int64_t windows);
-/* Device time of the last b2w_vad_probs call in milliseconds: window kernel, recurrence, decoder (CUDA events). */
+/* Device time of the last b2w_vad_probs or b2w_vad_probs_multi call in milliseconds: window kernel, recurrence, decoder
+ * (CUDA events), summed over its launches. */
 int b2w_vad_timing(b2w_vad* vad, double ms_out[3]);
 
 /* ---- measurement --------------------------------------------------------------------------------
