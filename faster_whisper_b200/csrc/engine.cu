@@ -1187,7 +1187,7 @@ static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const in
     B2W_CHECK(bstep_xpart_floats(bs) <= m->d_xpart_floats, "cross-attention partial buffer");
     bs.layers = m->d_blayers; bs.tok_emb = m->tok_emb; bs.pos_emb = m->dec_pos;
     bs.logit_atoms = m->logit_atoms; bs.logit_bias = m->logit_b; bs.logit_scale = m->logit_scale;
-    if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // read per call: tools/bstep_bisect.py steps it
+    if (const char* v = getenv("B2W_BSTEP_STOP")) bs.stop_phase = atoi(v);  // read per call: tests/test_gpu_decode_phases.py steps it
     bs.rows = sb.rows; bs.tokens_in = sb.tokens_in;
     bs.x = m->d_x; bs.ao = m->d_ao; bs.h16 = m->d_h16; bs.xn16 = m->d_xn16;
     bs.stats = m->d_stats; bs.stpart = m->d_stpart; bs.gpart = m->d_gpart; bs.logits = m->d_logits;
@@ -2257,26 +2257,108 @@ int b2w_debug_fetch(b2w_model* h, int32_t which, float* out, int64_t n) {
     B2W_CHECK(out && n >= 0, "null argument");
     B2W_CHECK(m->d_x, "no decoder workspace yet");
     B2W_CUDA(cudaStreamSynchronize(m->stream));
+    const b2w_config& c = m->cfg;
+    const int64_t dt = c.n_text_state, L = c.n_text_layer;
     const float* f32 = nullptr;
     const __half* f16 = nullptr;
+    int64_t size = 0, rows = 1, pitch = 0;  // the buffer's elements; the caches are copied as L rows of n / L elements, kv_elems apart
     switch (which) {
-      case 0: f32 = m->d_x; break;
-      case 1: f32 = m->d_gpart; break;
-      case 2: f32 = m->d_stpart; break;
-      case 4: f16 = m->d_ao; break;
-      case 5: f16 = m->d_h16; break;
-      case 6: f16 = m->d_xn16; break;
-      case 7: f32 = m->d_stats; break;
-      case 8: f32 = m->d_logits; break;
+      case 0: f32 = m->d_x; size = (int64_t)kMaxRows * ceil_div((int)dt, 128) * 128; break;
+      case 1: f32 = m->d_gpart; size = (int64_t)m->num_sms * kMaxRows * 128; break;
+      case 2: f32 = m->d_stpart; size = dt / 64 * kMaxRows * 2; break;
+      case 4: f16 = m->d_ao; size = kMaxRows * dt; break;
+      case 5: f16 = m->d_h16; size = kMaxRows * 4 * dt; break;
+      case 6: f16 = m->d_xn16; size = kMaxRows * dt; break;
+      case 7: f32 = m->d_stats; size = 3 * L * kMaxRows * 2; break;
+      case 8: f32 = m->d_logits; size = (int64_t)kMaxRows * m->vpad; break;
+      case 9:
+      case 10:
+        B2W_CHECK(m->kcache, "no self-attention cache yet");
+        f16 = which == 9 ? m->kcache : m->vcache;
+        B2W_CHECK(n % L == 0, "the caches are fetched as L equal per-layer prefixes");
+        size = L * (int64_t)m->kv_elems;
+        rows = L;
+        pitch = (int64_t)m->kv_elems;
+        break;
+      case 11:
+        B2W_CHECK(m->h_bind.xkv, "no encoder output bound");
+        f16 = m->h_bind.xkv;
+        size = L * 2 * m->h_bind.B_total * 1500 * dt;
+        break;
       default: throw Error("b2w_debug_fetch: unknown buffer", true);
     }
+    B2W_CHECK(n / rows <= (pitch ? pitch : size), "n exceeds the buffer");
+    if (n == 0) return;
     if (f32) {
       B2W_CUDA(cudaMemcpy(out, f32, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
     } else {
       std::vector<__half> tmp((size_t)n);
-      B2W_CUDA(cudaMemcpy(tmp.data(), f16, (size_t)n * sizeof(__half), cudaMemcpyDeviceToHost));
+      const size_t w = (size_t)(n / rows) * sizeof(__half);
+      B2W_CUDA(cudaMemcpy2D(tmp.data(), w, f16, (size_t)(pitch ? pitch : n) * sizeof(__half), w, (size_t)rows, cudaMemcpyDeviceToHost));
       for (int64_t i = 0; i < n; ++i) out[i] = __half2float(tmp[(size_t)i]);
     }
+  });
+}
+
+int b2w_debug_self_attn(int32_t device, const uint16_t* q, const uint16_t* kcache, const uint16_t* vcache, const uint8_t* anc,
+                        const int32_t* rows, int32_t R, int32_t H, int32_t n_chunks, int32_t slots, int32_t n_ctx, uint16_t* out) {
+  return guarded([&] {
+    B2W_CHECK(q && kcache && vcache && anc && rows && out, "null argument");
+    B2W_CHECK(R >= 1 && R <= 65535, "R must be in 1..65535");
+    B2W_CHECK(H >= 1 && H <= 20, "heads must be in 1..20");
+    B2W_CHECK(n_chunks >= 1 && slots >= 1 && slots <= kMaxBeam, "n_chunks >= 1 and slots in 1..16");
+    B2W_CHECK(n_ctx >= 1 && n_ctx <= B2W_MAX_TEXT_CTX, "n_ctx must be in 1..448");
+    const int d = 64 * H;
+    const size_t n_anc = (size_t)2 * n_chunks * slots * n_ctx, cache = (size_t)n_chunks * n_ctx * slots * d;
+    for (int r = 0; r < R; ++r)
+      B2W_CHECK(rows[4 * r] >= 0 && rows[4 * r] < n_chunks && rows[4 * r + 1] >= 0 && rows[4 * r + 1] < slots && rows[4 * r + 2] >= 0 &&
+                    rows[4 * r + 2] < n_ctx,
+                "row table entry outside the cache");
+    for (size_t i = 0; i < n_anc; ++i) B2W_CHECK(anc[i] < slots, "ancestry slot out of range");
+    require_hopper(device);
+    DeviceGuard g(device);
+    ScratchBufs sb;
+    SelfAttnArgs a;
+    a.rows = reinterpret_cast<const RowInfo*>(sb.put<int32_t>(rows, (size_t)4 * R));
+    a.q = sb.put<__half>(q, (size_t)R * d);
+    a.kcache = sb.put<__half>(kcache, cache);
+    a.vcache = sb.put<__half>(vcache, cache);
+    a.anc = sb.put<uint8_t>(anc, n_anc);
+    __half* o = sb.alloc<__half>((size_t)R * d);
+    a.out = o;
+    a.d = d; a.n_ctx = n_ctx; a.slots = slots;
+    a.anc_buf_stride = (long long)n_chunks * slots * n_ctx;
+    dec_self_attn(a, R, H, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    hook_get(out, o, (size_t)R * d * 2);
+  });
+}
+
+int b2w_debug_cross_attn(int32_t device, const uint16_t* q, const uint16_t* kv, int32_t n_chunks, int32_t rows_per_chunk, int32_t H,
+                         uint16_t* out) {
+  return guarded([&] {
+    B2W_CHECK(q && kv && out, "null argument");
+    B2W_CHECK(n_chunks >= 1 && n_chunks <= 16, "n_chunks must be in 1..16");
+    B2W_CHECK(rows_per_chunk >= 1 && rows_per_chunk <= kMaxBeam, "rows_per_chunk must be in 1..16");
+    B2W_CHECK(H >= 1 && H <= 20, "heads must be in 1..20");
+    require_hopper(device);
+    DeviceGuard g(device);
+    dstep_configure();  // per-device kernel attributes (build_model does this for real models)
+    const int d = 64 * H, R = n_chunks * rows_per_chunk, T = 1500;
+    const size_t groups = (size_t)n_chunks * H * ds_xqgroups(rows_per_chunk);
+    ScratchBufs sb;
+    const DecBindings bind{sb.put<__half>(kv, (size_t)2 * n_chunks * H * T * 64), n_chunks, 0};
+    DStepArgs a{};
+    a.q = sb.put<__half>(q, (size_t)R * d);
+    __half* o = sb.alloc<__half>((size_t)R * d);
+    a.ao = o;
+    a.bind = sb.put<DecBindings>(&bind, 1);
+    a.xpart = sb.alloc<float>(groups * kDsXSplits * kDsXQ * 66);
+    a.xcounters = sb.put<int>(nullptr, 0, groups);
+    a.H = H; a.T = T; a.d = d; a.rows_per_chunk = rows_per_chunk; a.n_chunks = n_chunks;
+    dstep_cross_attn_launch(a, 0, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    hook_get(out, o, (size_t)R * d * 2);
   });
 }
 

@@ -146,7 +146,7 @@ ABI_SYMBOLS = (
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
     "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
-    "b2w_debug_step_logits", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
+    "b2w_debug_step_logits", "b2w_debug_self_attn", "b2w_debug_cross_attn", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
 )
 
 
@@ -208,6 +208,9 @@ def load_library():
         lib.b2w_debug_fetch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
         lib.b2w_debug_step_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                               C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.b2w_debug_self_attn.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+        lib.b2w_debug_cross_attn.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         lib.b2w_debug_search.argtypes = [C.c_int32, C.POINTER(_SearchDesc)]
         lib.b2w_debug_align_cost.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                              C.c_void_p]
@@ -935,6 +938,37 @@ def debug_dtw(cost: np.ndarray, capacity: Optional[int] = None, device: int = 0)
     n = C.c_int32(0)
     _check(lib.b2w_debug_dtw(device, _ptr(c), N, M, _ptr(pairs), cap, C.byref(n)))
     return [(int(a), int(b)) for a, b in pairs[: n.value]]
+
+
+def debug_self_attn(q: np.ndarray, kcache: np.ndarray, vcache: np.ndarray, anc: np.ndarray, rows: np.ndarray, device: int = 0) -> np.ndarray:
+    """The decoder's masked self-attention kernel (tests only): q float16 [R, 64 H], caches float16 [n_chunks, n_ctx, slots, 64 H],
+    anc uint8 [2, n_chunks, slots, n_ctx] (a row at position p reads buffer p & 1), rows int32 [R, 4] = (chunk, slot, pos, -).
+    Returns float16 [R, 64 H]."""
+    lib = load_library()
+    q, kcache, vcache = (np.ascontiguousarray(x, np.float16) for x in (q, kcache, vcache))
+    anc, rows = np.ascontiguousarray(anc, np.uint8), np.ascontiguousarray(rows, np.int32)
+    if q.ndim != 2 or q.shape[1] % 64 or kcache.ndim != 4 or kcache.shape != vcache.shape or kcache.shape[3] != q.shape[1]:
+        raise ValueError("q must be [R, 64 H] and both caches [n_chunks, n_ctx, slots, 64 H]")
+    n_chunks, n_ctx, slots, _ = kcache.shape
+    if anc.shape != (2, n_chunks, slots, n_ctx) or rows.shape != (q.shape[0], 4):
+        raise ValueError("anc must be [2, n_chunks, slots, n_ctx] and rows [R, 4]")
+    out = np.zeros_like(q)
+    _check(lib.b2w_debug_self_attn(device, _ptr(q), _ptr(kcache), _ptr(vcache), _ptr(anc), _ptr(rows), q.shape[0], q.shape[1] // 64,
+                                   n_chunks, slots, n_ctx, _ptr(out)))
+    return out
+
+
+def debug_cross_attn(q: np.ndarray, kv: np.ndarray, device: int = 0) -> np.ndarray:
+    """The decoder's beam-shared cross-attention kernel (tests only): q float16 [n_chunks, rows_per_chunk, 64 H], kv float16
+    [2, n_chunks, H, 1500, 64] as the encoder output stores it (16-byte chunk c of key t at c ^ (t & 7)).  Returns float16
+    [n_chunks, rows_per_chunk, 64 H]."""
+    lib = load_library()
+    q, kv = np.ascontiguousarray(q, np.float16), np.ascontiguousarray(kv, np.float16)
+    if q.ndim != 3 or kv.ndim != 5 or kv.shape[0] != 2 or kv.shape[1] != q.shape[0] or kv.shape[3:] != (1500, 64) or q.shape[2] != 64 * kv.shape[2]:
+        raise ValueError("q must be [n_chunks, rows_per_chunk, 64 H] and kv [2, n_chunks, H, 1500, 64]")
+    out = np.zeros_like(q)
+    _check(lib.b2w_debug_cross_attn(device, _ptr(q), _ptr(kv), q.shape[0], q.shape[1], kv.shape[2], _ptr(out)))
+    return out
 
 
 def debug_gemv(x: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: int = 0, device: int = 0):

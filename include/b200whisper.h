@@ -330,9 +330,21 @@ int b2w_debug_dtw(int32_t device, const double* cost, int32_t N, int32_t M, int3
 /* decoder workspace of the last decode step as float32 (fp16 buffers are widened): which = 0 residual stream [R][d], 1 the
  * many-row step kernel's split-K partial tiles of its last GEMM phase [CTA][R][128], 2 the per-k-atom partials of its last row
  * statistics [d/64][R][2], 4 attention output [R][d], 5 GELU(hidden) [R][4d], 6 final LayerNorm output [R][d], 7 LayerNorm
- * statistics [3L][80][2], 8 logits [R][vpad]; n = number of floats to copy.
+ * statistics [3L][R][2], 8 logits [R][vpad], 9 / 10 the self-attention K / V cache of every layer [L][chunk][n_ctx][slot][d]
+ * (n / L elements from the start of each layer's cache), 11 the cross-attention K/V of the encoder output the last step read
+ * [L][2][B][H][1500][64] (16-byte chunk c of key t at c ^ (t & 7)); n = number of floats to copy, at most the buffer's size.
  * With B2W_BSTEP_STOP=<p> the many-row step kernel stops after p grid phases, so this bisects it phase by phase. */
 int b2w_debug_fetch(b2w_model* m, int32_t which, float* out, int64_t n);
+/* The decoder's masked self-attention kernel on fp16 inputs: rows [R][4] = (chunk, slot, pos, -), q [R][64 H], kcache / vcache
+ * [n_chunks][n_ctx][slots][64 H], anc [2][n_chunks][slots][n_ctx]: row r reads buffer pos & 1, key j < pos from slot
+ * anc[pos & 1][chunk][slot][j] and key pos from its own slot.  out [R][64 H] fp16.  Arguments are checked before any device work. */
+int b2w_debug_self_attn(int32_t device, const uint16_t* q, const uint16_t* kcache, const uint16_t* vcache, const uint8_t* anc,
+                        const int32_t* rows, int32_t R, int32_t H, int32_t n_chunks, int32_t slots, int32_t n_ctx, uint16_t* out);
+/* The decoder's beam-shared cross-attention kernel on fp16 inputs: q [n_chunks * rows_per_chunk][64 H] (row b * rows_per_chunk + i
+ * of chunk b), kv [2][n_chunks][H][1500][64] one layer's K and V as the encoder output stores them (16-byte chunk c of key t at
+ * c ^ (t & 7)).  out [n_chunks * rows_per_chunk][64 H] fp16.  Arguments are checked before any device work. */
+int b2w_debug_cross_attn(int32_t device, const uint16_t* q, const uint16_t* kv, int32_t n_chunks, int32_t rows_per_chunk, int32_t H,
+                         uint16_t* out);
 
 #ifdef __cplusplus
 }

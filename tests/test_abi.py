@@ -57,6 +57,38 @@ def test_gemm_hooks_check_arguments_before_the_device():
         engine.debug_gemv_desc(np.zeros((81, 64), np.float16), w, mode=engine.GV_F32, out=np.zeros(81 * 128, np.float32), ldo=128)
 
 
+def test_attention_hooks_check_arguments_before_the_device():
+    """Bad inputs of the decoder attention hooks are refused (ValueError) before anything touches a device, GPU or not."""
+    q, kc = np.zeros((2, 128), np.float16), np.zeros((1, 8, 4, 128), np.float16)
+    anc, rows = np.zeros((2, 1, 4, 8), np.uint8), np.array([[0, 1, 3, 0], [0, 3, 7, 0]], np.int32)
+    for r, field, v in ((1, 2, 8), (0, 1, 4), (1, 0, 1), (0, 2, -1)):
+        bad = rows.copy()
+        bad[r, field] = v
+        with pytest.raises(ValueError, match="row table"):
+            engine.debug_self_attn(q, kc, kc.copy(), anc, bad)
+    bad = anc.copy()
+    bad[1, 0, 2, 5] = 4
+    with pytest.raises(ValueError, match="ancestry slot"):
+        engine.debug_self_attn(q, kc, kc.copy(), bad, rows)
+    with pytest.raises(ValueError, match="slots in 1..16"):
+        engine.debug_self_attn(q, np.zeros((1, 8, 17, 128), np.float16), np.zeros((1, 8, 17, 128), np.float16),
+                               np.zeros((2, 1, 17, 8), np.uint8), rows)
+    with pytest.raises(ValueError, match="n_ctx"):
+        engine.debug_self_attn(q, np.zeros((1, 449, 4, 128), np.float16), np.zeros((1, 449, 4, 128), np.float16),
+                               np.zeros((2, 1, 4, 449), np.uint8), rows)
+    with pytest.raises(ValueError, match="caches"):
+        engine.debug_self_attn(q[:, :64], kc, kc.copy(), anc, rows)
+    kv = np.zeros((2, 17, 1, 1500, 64), np.float16)
+    with pytest.raises(ValueError, match="n_chunks"):
+        engine.debug_cross_attn(np.zeros((17, 1, 64), np.float16), kv)
+    with pytest.raises(ValueError, match="rows_per_chunk"):
+        engine.debug_cross_attn(np.zeros((1, 17, 64), np.float16), kv[:, :1])
+    with pytest.raises(ValueError, match="heads"):
+        engine.debug_cross_attn(np.zeros((1, 1, 21 * 64), np.float16), np.zeros((2, 1, 21, 1500, 64), np.float16))
+    with pytest.raises(ValueError, match="kv"):
+        engine.debug_cross_attn(np.zeros((1, 1, 64), np.float16), np.zeros((2, 1, 1, 1499, 64), np.float16))
+
+
 def test_search_hook_checks_arguments_before_the_device():
     """Bad search-step descriptors are refused (ValueError) before anything touches a device, GPU or not."""
     from faster_whisper_b200.config import special_tokens
