@@ -217,9 +217,9 @@ __device__ __forceinline__ void bs_issue_cross_kv(const BStepArgs& a, int layer,
   const int split = task % kDsXSplits, rest = task / kDsXSplits;
   const int h = rest % a.H, b = rest / a.H, T = a.T;
   const int k0 = T * split / kDsXSplits, k1 = T * (split + 1) / kDsXSplits, nk = k1 - k0;
-  const DecBindings bd = *a.bind;
+  const DecBindings bd = a.bind[b];
   const long long per = (long long)bd.B_total * a.H * T * 64;
-  const long long off = (((long long)(bd.chunk0 + b) * a.H + h) * T + k0) * 64;
+  const long long off = (((long long)bd.item * a.H + h) * T + k0) * 64;
   const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + off;
   const __half* Vb = bd.xkv + ((long long)layer * 2 + 1) * per + off;
   fence_proxy_async();

@@ -46,7 +46,7 @@ struct BStepArgs {
   long long kv_layer_stride;
   const uint8_t* anc;
   long long anc_buf_stride;
-  const DecBindings* bind;
+  const DecBindings* bind;  // [n_chunks] encoder binding of each chunk
   float* xpart;
   int* xcounters;
   unsigned* bar;  // [kBsBarWords]: grid barrier, then from word 64 the n-block group counters [6 matrices][64 n-blocks]

@@ -52,12 +52,13 @@ struct SelfAttnArgs {
 };
 void dec_self_attn(const SelfAttnArgs& a, int R, int H, cudaStream_t s);
 
-// Per-generate-call bindings read by the step kernels from device memory, so that the captured CUDA graph of a
-// decode step does not depend on which encoder output (or which slice of it) is being decoded.
+// Encoder binding of one decode chunk (one entry per chunk of a pass or slot of a step, in device memory): the chunk attends to
+// item `item` of an encoder output whose cross-attention K/V is xkv.  The step kernels read their chunk's entry, so the captured
+// CUDA graph of a decode step does not depend on which encoder outputs (or which items of them) the chunks decode.
 struct DecBindings {
   const __half* xkv;  // [L][2][B_total][H][T][64]
   int B_total;
-  int chunk0;
+  int item;
 };
 
 void search_configure();  // per-device kernel attributes (must run outside stream capture)
@@ -75,8 +76,6 @@ struct SearchParams {
   int B, K;                    // chunks, rows per chunk
   int mode;                    // 0 beam, 1 greedy/sampling (independent rows)
   int ncand;                   // beam: 2K ; greedy: 1
-  int max_steps;               // generated tokens allowed (max_length - prompt_len)
-  int prompt_len;
   int max_finished;            // round(K * patience), at most kMaxFinishTarget
   int allow_early_exit;
   int num_hyp;
@@ -85,14 +84,31 @@ struct SearchParams {
   int suppress_blank;
   int n_suppress_begin;
   int suppress_begin[8];
-  int timestamp_rules;
   int max_initial_ts;
   int eot, no_timestamps, timestamp_begin, no_speech;
   int sampling_topk;
   float temperature;
   unsigned long long seed;
-  int want_no_speech_first;    // no_speech prob comes from the first decode step (sot is the last prompt token)
   int fake_logits;
+};
+
+// Per-chunk search state that a decode session changes when it gives a slot to a new item.
+struct ChunkParams {
+  int prompt_len;
+  int max_steps;               // generated tokens allowed (max_length - prompt_len)
+  int item;                    // keys the sampling noise with the row within the chunk, so draws do not depend on the slot
+  int timestamp_rules;         // the prompt has no <|notimestamps|>
+  int ns_first;                // no_speech prob comes from the first decode step (sot is the last prompt token)
+  int pad[3];
+};
+
+// A slot's new occupant: search_reset_slots clears the slot's search state and starts its rows at the prompt's last token.
+struct SlotReset {
+  int slot;
+  int last_token;
+  int done;                    // 1: the slot stays idle (counted as done)
+  int pad;
+  ChunkParams cp;
 };
 
 // All mutable search state lives on the device so a decode step needs no host round trip.
@@ -106,6 +122,7 @@ struct SearchState {
 struct SearchBuffers {
   SearchState* state;          // [1]
   const SearchParams* params;  // [1] device copy of the options of the running generate() call
+  ChunkParams* chunk;          // [B]
   RowInfo* rows;               // [B*K]
   int* tokens_in;              // [B*K] token fed at this step
   float* cum;                  // [2][B*K]
@@ -127,16 +144,18 @@ struct SearchBuffers {
 // `p` lives in device memory (SearchBuffers::params) so a captured step graph is independent of the options
 void search_rows(const float* logits, int R, int vpad, const SearchBuffers& b, cudaStream_t s);
 void search_update(int B, const SearchBuffers& b, cudaStream_t s);
+// resets slot resets[i].slot of a B x K search for its new occupant; the other slots are not touched
+void search_reset_slots(const SlotReset* resets, int n, int B, int K, const SearchBuffers& b, cudaStream_t s);
 void fake_logits(float* logits, int R, const SearchBuffers& b, cudaStream_t s);
 void no_speech_from_logits(const float* logits, int row_stride, int R, int rows_per_chunk, int row_in_chunk, int n_vocab,
                            int no_speech_id, float* out, cudaStream_t s);
 void lang_probs_from_logits(const float* logits, int row_stride, int B, int lang_begin, int n_lang, float* out, cudaStream_t s);
 // Whisper.align helpers (search.cu)
 void row_target_probs(const float* logits, int row_stride, int R, int n_vocab, const int* targets, float* out, cudaStream_t s);
-// Row r of the pass writes out[rows[r].chunk][head][rows[r].pos][0..nf) of an [items][n_heads][n_tok][nf] capture, with the keys
-// of encoder chunk bind->chunk0 + rows[r].chunk.
+// Row r of the pass (chunk b = r / rows_per_chunk) writes out[b][head][rows[r].pos][0..nf) of an [items][n_heads][n_tok][nf]
+// capture, with the keys of the encoder item bind[b] names.
 void align_probs(const __half* q, const DecBindings* bind, const RowInfo* rows, int layer, const int2* heads, int n_heads, float* out,
-                 int n_tok, int nf, int R, int H, int T, int d, cudaStream_t s);
+                 int n_tok, int nf, int R, int rows_per_chunk, int H, int T, int d, cudaStream_t s);
 
 // ---- Whisper.align post-processing (align.cu) ----------------------------------------------------------------------------
 constexpr int kAlignMaxRows = 449;  // DTW rows (n_text + 1) the kernels take: more than a 448-position decoder can force

@@ -423,9 +423,9 @@ __device__ __noinline__ void ds_issue_cross_kv(const DStepArgs& a, DsShared& sh,
   const int split = task % kDsXSplits, bh = task / kDsXSplits / ds_xqgroups(a.rows_per_chunk);
   const int h = bh % a.H, b = bh / a.H, T = a.T;
   const int k0 = (int)((long long)T * split / kDsXSplits), k1 = (int)((long long)T * (split + 1) / kDsXSplits), nk = k1 - k0;
-  const DecBindings bd = *a.bind;
+  const DecBindings bd = a.bind[b];
   const long long per = (long long)bd.B_total * a.H * T * 64;
-  const long long off = (((long long)(bd.chunk0 + b) * a.H + h) * T + k0) * 64;
+  const long long off = (((long long)bd.item * a.H + h) * T + k0) * 64;
   const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + off;
   const __half* Vb = bd.xkv + ((long long)layer * 2 + 1) * per + off;
   fence_proxy_async();  // the buffer was last written through the generic proxy (self-attention staging)

@@ -36,7 +36,7 @@ struct DStepArgs {
   long long kv_layer_stride;
   const uint8_t* anc;
   long long anc_buf_stride;
-  const DecBindings* bind;
+  const DecBindings* bind;  // [n_chunks] encoder binding of each chunk
   float* xpart;
   int* xcounters;
   unsigned* bar;

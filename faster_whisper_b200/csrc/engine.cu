@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <deque>
 #include <cmath>
 #include <limits>
 #include <numeric>
@@ -16,6 +17,8 @@
 namespace b2w {
 
 // ---- error / counters ---------------------------------------------------------------------------------------
+constexpr int kMaxRows = 80;  // decode rows of one step or forced pass (chunks x rows per chunk)
+
 static thread_local std::string g_last_error;
 static thread_local int64_t g_launches = 0;
 void count_launch(int n) { g_launches += n; }
@@ -473,7 +476,7 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
   B2W_CUDA(cudaMemset(m->d_counters, 0, (64 + 16 * 20 * 64) * sizeof(int)));
   B2W_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->h_pinned), 4096));
   m->d_suppress = model_alloc<uint8_t>(m, m->vpad);
-  m->d_bind = model_alloc<DecBindings>(m, 1);
+  m->d_bind = model_alloc<DecBindings>(m, kMaxRows);
   search_configure();
   gemm_configure();
   dstep_configure();
@@ -737,7 +740,6 @@ static std::unique_ptr<Encoded> encode(Model* m, int B, F&& fill) {
 static int mel_frames(int64_t n_samples) { return (int)(1 + n_samples / 160); }
 
 // ---- decoder ----------------------------------------------------------------------------------------------------------------
-constexpr int kMaxRows = 80;
 constexpr size_t kCrossGroupCounters = 16 * 20 * 64;  // (chunk, head, query group) counters of the layered cross-attention
 
 static void ensure_decoder_ws(Model* m, int chunks, int slots) {
@@ -792,7 +794,7 @@ static void ensure_search_ws(Model* m, int B, int K) {
     return o;
   };
   const size_t Rr = std::max<size_t>(R, kMaxRows);
-  const size_t o_params = take(sizeof(SearchParams));
+  const size_t o_params = take(sizeof(SearchParams)), o_chunk = take(B * sizeof(ChunkParams));
   const size_t o_state = take(sizeof(SearchState)), o_rows = take(Rr * sizeof(RowInfo)), o_tok = take(Rr * 4),
                o_cum = take(2 * R * 4), o_hist = take(2 * R * n_ctx * 4), o_anc = take(2 * R * n_ctx),
                o_cs = take(R * kMaxCand * 4), o_ct = take(R * kMaxCand * 4), o_done = take(B * 4), o_fc = take(B * 4),
@@ -803,6 +805,7 @@ static void ensure_search_ws(Model* m, int B, int K) {
   SearchBuffers& sb = m->sb;
   sb.state = reinterpret_cast<SearchState*>(blob + o_state);
   sb.params = reinterpret_cast<const SearchParams*>(blob + o_params);
+  sb.chunk = reinterpret_cast<ChunkParams*>(blob + o_chunk);
   sb.rows = reinterpret_cast<RowInfo*>(blob + o_rows);
   sb.tokens_in = reinterpret_cast<int*>(blob + o_tok);
   sb.cum = reinterpret_cast<float*>(blob + o_cum);
@@ -927,9 +930,19 @@ static void gv(Model* m, GvArgs a) {
     skinny_gemm(a, m->stream);
 }
 
-static void bind_encoded(Model* m, const Encoded* e, int chunk0) {
-  m->h_bind = DecBindings{e ? e->xkv : nullptr, e ? e->B : 0, chunk0};
-  B2W_CUDA(cudaMemcpyAsync(m->d_bind, &m->h_bind, sizeof(DecBindings), cudaMemcpyHostToDevice, m->stream));
+// Uploads the encoder binding of every chunk of the next pass or step (entry b for chunk b).
+static void bind_chunks(Model* m, const std::vector<DecBindings>& bind) {
+  B2W_CHECK(!bind.empty() && bind.size() <= (size_t)kMaxRows, "decode chunks");
+  m->h_binds = bind;
+  m->h_bind = bind[0];
+  B2W_CUDA(cudaMemcpyAsync(m->d_bind, m->h_binds.data(), bind.size() * sizeof(DecBindings), cudaMemcpyHostToDevice, m->stream));
+}
+
+// Bindings of items chunk0 .. chunk0 + n - 1 of `e` (null for fake logits) to chunks 0 .. n - 1.
+static std::vector<DecBindings> item_range(const Encoded* e, int chunk0, int n) {
+  std::vector<DecBindings> bind(n);
+  for (int b = 0; b < n; ++b) bind[b] = DecBindings{e ? e->xkv : nullptr, e ? e->B : 0, chunk0 + b};
+  return bind;
 }
 
 // Floats of the cross-attention partial buffer for n_chunks x rows_per_chunk rows: 64 outputs + max + sum per (chunk, head,
@@ -958,8 +971,9 @@ struct AlignCapture {
 };
 
 // The layered decoder step: one launch per GEMM / attention.  Needs ensure_xpart(m, xpart_floats(m, n_chunks, rows_per_chunk)).
-// Every LayerNorm normalises only: the affines are folded into the projections that consume them (fold_ln).
-static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots, const AlignCapture* cap) {
+// Every LayerNorm normalises only: the affines are folded into the projections that consume them (fold_ln).  The slot ancestry
+// buffers hold anc_chunks chunks.
+static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots, int anc_chunks, const AlignCapture* cap) {
   const b2w_config& c = m->cfg;
   const int dt = c.n_text_state, L = c.n_text_layer, H = c.n_text_head, R = n_chunks * rows_per_chunk;
   cudaStream_t s = m->stream;
@@ -975,7 +989,7 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     a.x = m->d_xn; a.W = W.wqkv; a.bias = W.bqkv; a.R = R; a.N = 3 * dt; a.K = dt; a.mode = GV_QKV;
     a.rows = sb.rows; a.kcache = kc; a.vcache = vc; a.d = dt; a.n_ctx = c.n_text_ctx; a.slots = slots; a.out_h = m->d_q;
     gv(m, a);
-    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots, (long long)n_chunks * slots * c.n_text_ctx};
+    SelfAttnArgs sa{sb.rows, m->d_q, kc, vc, sb.anc, m->d_ao, dt, c.n_text_ctx, slots, (long long)anc_chunks * slots * c.n_text_ctx};
     dec_self_attn(sa, R, H, s);
     GvArgs o;
     o.x = m->d_ao; o.W = W.wo; o.bias = W.bo; o.R = R; o.N = dt; o.K = dt; o.mode = GV_RESID_LN;
@@ -984,7 +998,7 @@ static void decoder_layers(Model* m, int n_chunks, int rows_per_chunk, int slots
     GvArgs q;
     q.x = m->d_xn; q.W = W.wq_x; q.bias = W.bq_x; q.R = R; q.N = dt; q.K = dt; q.mode = GV_F16; q.out_h = m->d_q;
     gv(m, q);
-    if (cap) align_probs(m->d_q, m->d_bind, sb.rows, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, R, H, 1500, dt, s);
+    if (cap) align_probs(m->d_q, m->d_bind, sb.rows, l, cap->heads, cap->n_heads, cap->out, cap->n_tok, cap->nf, R, rows_per_chunk, H, 1500, dt, s);
     DStepArgs xa{};
     xa.q = m->d_q; xa.ao = m->d_ao; xa.bind = m->d_bind; xa.xpart = m->d_xpart; xa.xcounters = m->d_counters + 64;
     xa.H = H; xa.T = 1500; xa.d = dt; xa.rows_per_chunk = rows_per_chunk; xa.n_chunks = n_chunks;
@@ -1012,14 +1026,30 @@ static void logits_gemm(Model* m, int R) {
 
 static int forced_positions_per_pass(int n_chunks) { return std::max(1, kMaxRows / n_chunks); }
 
-// Forced decoding of tokens[b * stride + i], i < n_tok, for chunks chunk0 .. chunk0+n of `e`, in passes of
-// forced_positions_per_pass(n) positions; every row writes self-KV slot 0 of `slots`.  The slot ancestry must be zero: clear_anc
-// zeroes it, unless the caller already has.  When `cap` is set, every pass captures the alignment heads' cross-attention.
-// After each pass's decoder layers, on_pass(i0, i1) may run logits_gemm: row b * (i1 - i0) + (i - i0) holds position i of chunk b.
+// The chunks of a forced decoding: chunk b attends to the encoder item bind[b] and writes its keys as chunk kv_chunk[b] of a
+// self-KV cache (and slot ancestry) of anc_chunks chunks.
+struct ForcedChunks {
+  std::vector<DecBindings> bind;
+  std::vector<int> kv_chunk;
+  int anc_chunks;
+};
+
+// Items chunk0 .. chunk0 + n - 1 of `e` as chunks 0 .. n - 1 of their own cache.
+static ForcedChunks forced_range(const Encoded* e, int chunk0, int n) {
+  ForcedChunks fc{item_range(e, chunk0, n), std::vector<int>(n), n};
+  for (int b = 0; b < n; ++b) fc.kv_chunk[b] = b;
+  return fc;
+}
+
+// Forced decoding of tokens[b * stride + i], i < n_tok, for the chunks of fc, in passes of forced_positions_per_pass(n)
+// positions; every row writes self-KV slot 0 of `slots`.  The slot ancestry must be zero: clear_anc zeroes it, unless the caller
+// already has.  When `cap` is set, every pass captures the alignment heads' cross-attention.  After each pass's decoder layers,
+// on_pass(i0, i1) may run logits_gemm: row b * (i1 - i0) + (i - i0) holds position i of chunk b.
 template <typename F>
-static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const int32_t* tokens, int stride, int n_tok, int slots,
-                          bool clear_anc, const AlignCapture* cap, F&& on_pass) {
-  if (clear_anc) B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * n * slots * m->cfg.n_text_ctx, m->stream));
+static void forced_decode(Model* m, const ForcedChunks& fc, const int32_t* tokens, int stride, int n_tok, int slots, bool clear_anc,
+                          const AlignCapture* cap, F&& on_pass) {
+  const int n = (int)fc.bind.size();
+  if (clear_anc) B2W_CUDA(cudaMemsetAsync(m->sb.anc, 0, (size_t)2 * fc.anc_chunks * slots * m->cfg.n_text_ctx, m->stream));
   const int per_pass = forced_positions_per_pass(n);
   for (int i0 = 0; i0 < n_tok; i0 += per_pass) {
     const int i1 = std::min(n_tok, i0 + per_pass), rpc = i1 - i0, R = n * rpc;
@@ -1027,15 +1057,15 @@ static void forced_decode(Model* m, const Encoded* e, int chunk0, int n, const i
     std::vector<int> toks(R);
     for (int b = 0; b < n; ++b)
       for (int i = i0; i < i1; ++i) {
-        rows[b * rpc + (i - i0)] = RowInfo{b, 0, i, 0};
+        rows[b * rpc + (i - i0)] = RowInfo{fc.kv_chunk[b], 0, i, 0};
         toks[b * rpc + (i - i0)] = tokens[(size_t)b * stride + i];
       }
     B2W_CUDA(cudaMemcpyAsync(m->sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, m->stream));
     B2W_CUDA(cudaMemcpyAsync(m->sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
     B2W_CUDA(cudaStreamSynchronize(m->stream));  // host vectors go out of scope
-    bind_encoded(m, e, chunk0);
+    bind_chunks(m, fc.bind);
     ensure_xpart(m, xpart_floats(m, n, rpc));
-    decoder_layers(m, n, rpc, slots, cap);
+    decoder_layers(m, n, rpc, slots, fc.anc_chunks, cap);
     on_pass(i0, i1);
   }
 }
@@ -1080,14 +1110,12 @@ static std::vector<uint8_t> suppress_mask(const b2w_config& c, int vpad, const b
   return mask;
 }
 
-static SearchParams search_params(const b2w_config& c, int vpad, const int32_t* prompts, int n, int K, int P, int sot_index,
-                                  const b2w_gen_opts& o) {
+static SearchParams search_params(const b2w_config& c, int vpad, int n, int K, const b2w_gen_opts& o) {
   const bool beam = o.beam_size > 1;
   SearchParams sp{};
   sp.n_vocab = c.n_vocab; sp.vpad = vpad; sp.B = n; sp.K = K;
   sp.mode = beam ? 0 : 1;
   sp.ncand = beam ? 2 * K : 1;
-  sp.max_steps = o.max_length - P; sp.prompt_len = P;
   sp.max_finished = std::max(1, (int)lroundf(K * o.patience));
   sp.allow_early_exit = (o.patience == 1.0f && o.length_penalty == 0.0f) ? 1 : 0;
   sp.num_hyp = std::max(1, o.num_hypotheses);
@@ -1096,14 +1124,10 @@ static SearchParams search_params(const b2w_config& c, int vpad, const int32_t* 
   sp.suppress_blank = o.suppress_blank;
   sp.n_suppress_begin = c.n_suppress_begin;
   for (int i = 0; i < 8; ++i) sp.suppress_begin[i] = c.suppress_begin[i];
-  bool has_no_ts = false;
-  for (int i = 0; i < P; ++i) has_no_ts = has_no_ts || prompts[i] == c.no_timestamps;
-  sp.timestamp_rules = has_no_ts ? 0 : 1;
   sp.max_initial_ts = o.max_initial_timestamp_index;
   sp.eot = c.eot; sp.no_timestamps = c.no_timestamps; sp.timestamp_begin = c.timestamp_begin; sp.no_speech = c.no_speech;
   sp.sampling_topk = o.sampling_topk; sp.temperature = o.sampling_temperature > 0 ? o.sampling_temperature : 1.0f;
   sp.seed = o.seed;
-  sp.want_no_speech_first = (o.return_no_speech_prob && sot_index == P - 1) ? 1 : 0;
   sp.fake_logits = o.debug_fake_logits;
   B2W_CHECK(sp.max_finished <= kMaxFinishTarget, "beam_size * patience is too large");
   // a chunk stops at max_finished, but the step that reaches it can finish up to K hypotheses: all must have a slot
@@ -1111,12 +1135,24 @@ static SearchParams search_params(const b2w_config& c, int vpad, const int32_t* 
   return sp;
 }
 
+// The search state of a chunk decoding `prompt` (P tokens, <|startoftranscript|> at sot_index) up to max_length tokens.
+static ChunkParams chunk_params(const b2w_config& c, const int32_t* prompt, int P, int sot_index, int max_length, int item,
+                                bool no_speech) {
+  ChunkParams cp{};
+  cp.prompt_len = P;
+  cp.max_steps = max_length - P;
+  cp.item = item;
+  cp.timestamp_rules = std::find(prompt, prompt + P, c.no_timestamps) == prompt + P ? 1 : 0;
+  cp.ns_first = (no_speech && sot_index == P - 1) ? 1 : 0;
+  return cp;
+}
+
 // Prompt[:-1] of every chunk of the group; the no-speech probability comes from the pass that holds the SOT row.  The search
 // reset has cleared the slot ancestry.
 static void prefill(Model* m, const Encoded* e, int chunk0, int n, const int32_t* prompts, int P, int K, int sot_index, bool no_speech) {
   ScopedStage st(m, B2W_T_PREFILL);
   const b2w_config& c = m->cfg;
-  forced_decode(m, e, chunk0, n, prompts + (size_t)chunk0 * P, P, P - 1, K, false, nullptr, [&](int i0, int i1) {
+  forced_decode(m, forced_range(e, chunk0, n), prompts + (size_t)chunk0 * P, P, P - 1, K, false, nullptr, [&](int i0, int i1) {
     if (!no_speech || sot_index < i0 || sot_index >= i1) return;
     logits_gemm(m, n * (i1 - i0));
     no_speech_from_logits(m->d_logits, m->vpad, n * (i1 - i0), i1 - i0, sot_index - i0, c.n_vocab, c.no_speech, m->sb.no_speech, m->stream);
@@ -1149,25 +1185,11 @@ static Step choose_step(const Model* m, int n, int K, bool fake_logits) {
   return st;
 }
 
-// Uploads the first decode rows, the search parameters and the encoder binding, sizes the partial buffer and binds the
-// workspace into the persistent kernel's argument block.
-static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const int32_t* prompts, int P, const SearchParams& sp) {
+// Sizes the partial buffer and binds the workspace into the persistent kernel's argument block.
+static void step_args(Model* m, Step& st) {
   const b2w_config& c = m->cfg;
   const int n = st.n, K = st.K, R = n * K;
-  cudaStream_t s = m->stream;
   const SearchBuffers& sb = m->sb;
-  {
-    std::vector<RowInfo> rows(R);
-    std::vector<int> toks(R);
-    for (int b = 0; b < n; ++b)
-      for (int k = 0; k < K; ++k) {
-        rows[b * K + k] = RowInfo{b, k, P - 1, 0};
-        toks[b * K + k] = prompts[(size_t)(chunk0 + b) * P + P - 1];
-      }
-    B2W_CUDA(cudaMemcpyAsync(sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, s));
-    B2W_CUDA(cudaMemcpyAsync(sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, s));
-    B2W_CUDA(cudaStreamSynchronize(s));
-  }
   if (st.path != StepPath::FakeLogits) ensure_xpart(m, xpart_floats(m, n, K));
   if (st.path == StepPath::Dstep) {
     DStepArgs& ds = st.ds;
@@ -1195,9 +1217,29 @@ static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const in
     bs.anc = sb.anc; bs.anc_buf_stride = (long long)n * K * c.n_text_ctx;
     bs.bind = m->d_bind; bs.xpart = m->d_xpart; bs.xcounters = m->d_counters + 64; bs.bar = m->d_bar; bs.prof = m->d_prof;
   }
+}
+
+// Uploads the first decode rows, the search parameters and the encoder binding, and fills the step's argument block.
+static void bind_step(Model* m, Step& st, const Encoded* e, int chunk0, const int32_t* prompts, int P, const SearchParams& sp) {
+  const int n = st.n, K = st.K, R = n * K;
+  cudaStream_t s = m->stream;
+  const SearchBuffers& sb = m->sb;
+  {
+    std::vector<RowInfo> rows(R);
+    std::vector<int> toks(R);
+    for (int b = 0; b < n; ++b)
+      for (int k = 0; k < K; ++k) {
+        rows[b * K + k] = RowInfo{b, k, P - 1, 0};
+        toks[b * K + k] = prompts[(size_t)(chunk0 + b) * P + P - 1];
+      }
+    B2W_CUDA(cudaMemcpyAsync(sb.rows, rows.data(), R * sizeof(RowInfo), cudaMemcpyHostToDevice, s));
+    B2W_CUDA(cudaMemcpyAsync(sb.tokens_in, toks.data(), R * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2W_CUDA(cudaStreamSynchronize(s));
+  }
+  step_args(m, st);
   m->h_params = sp;
   B2W_CUDA(cudaMemcpyAsync(const_cast<SearchParams*>(sb.params), &m->h_params, sizeof(SearchParams), cudaMemcpyHostToDevice, s));
-  bind_encoded(m, e, chunk0);
+  bind_chunks(m, item_range(e, chunk0, n));
 }
 
 // The decoder half of a step: the logits of every row into d_logits, from sb.rows, sb.tokens_in and sb.anc.
@@ -1208,7 +1250,7 @@ static void launch_decoder(Model* m, const Step& st) {
     case StepPath::Dstep: dstep_launch(st.ds, m->dstep_grid, m->stream); break;
     case StepPath::Bstep: bstep_launch(st.bs, m->num_sms, m->stream); break;
     case StepPath::Layers:
-      decoder_layers(m, st.n, st.K, st.K, nullptr);
+      decoder_layers(m, st.n, st.K, st.K, st.n, nullptr);
       logits_gemm(m, R);
       break;
   }
@@ -1279,8 +1321,8 @@ static void decode_loop(Model* m, const Step& st, int P, int max_steps) {
   if (m->d_prof && st.path == StepPath::Dstep) dstep_print_profile(st.ds, m->stream);
 }
 
-// Finished hypotheses of every chunk, best first by (length-penalised) score.
-static void collect_hypotheses(Model* m, int chunk0, int n, int K, const b2w_gen_opts& o, int32_t* out_ids, int32_t* out_lens,
+// Finished hypotheses of chunks slot0 .. slot0 + n - 1, best first by (length-penalised) score, into outputs chunk0 .. chunk0 + n - 1.
+static void collect_hypotheses(Model* m, int slot0, int chunk0, int n, int K, const b2w_gen_opts& o, int32_t* out_ids, int32_t* out_lens,
                                float* out_scores, float* out_ns) {
   ScopedStage st(m, B2W_T_D2H);
   cudaStream_t s = m->stream;
@@ -1290,11 +1332,11 @@ static void collect_hypotheses(Model* m, int chunk0, int n, int K, const b2w_gen
   std::vector<int> fin_count(n), fin_len((size_t)n * kMaxFinished);
   std::vector<float> fin_score((size_t)n * kMaxFinished), ns(n);
   std::vector<int> fin_tok((size_t)n * kMaxFinished * n_ctx);
-  B2W_CUDA(cudaMemcpyAsync(fin_count.data(), sb.fin_count, n * 4, cudaMemcpyDeviceToHost, s));
-  B2W_CUDA(cudaMemcpyAsync(fin_len.data(), sb.fin_len, fin_len.size() * 4, cudaMemcpyDeviceToHost, s));
-  B2W_CUDA(cudaMemcpyAsync(fin_score.data(), sb.fin_score, fin_score.size() * 4, cudaMemcpyDeviceToHost, s));
-  B2W_CUDA(cudaMemcpyAsync(fin_tok.data(), sb.fin_tok, fin_tok.size() * 4, cudaMemcpyDeviceToHost, s));
-  B2W_CUDA(cudaMemcpyAsync(ns.data(), sb.no_speech, n * 4, cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(fin_count.data(), sb.fin_count + slot0, n * 4, cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(fin_len.data(), sb.fin_len + (size_t)slot0 * kMaxFinished, fin_len.size() * 4, cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(fin_score.data(), sb.fin_score + (size_t)slot0 * kMaxFinished, fin_score.size() * 4, cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(fin_tok.data(), sb.fin_tok + (size_t)slot0 * kMaxFinished * n_ctx, fin_tok.size() * 4, cudaMemcpyDeviceToHost, s));
+  B2W_CUDA(cudaMemcpyAsync(ns.data(), sb.no_speech + slot0, n * 4, cudaMemcpyDeviceToHost, s));
   B2W_CUDA(cudaStreamSynchronize(s));
   for (int b = 0; b < n; ++b) {
     out_ns[chunk0 + b] = o.return_no_speech_prob ? ns[b] : 0.f;
@@ -1334,9 +1376,10 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
   const int K = o.beam_size > 1 ? o.beam_size : std::max(1, o.num_hypotheses);
   const int sot_index = validate_prompts(m->cfg, prompts + (size_t)chunk0 * P, n, P);
   for (int b = 0; b < n; ++b) out_ns[chunk0 + b] = 0.f;
-  const SearchParams sp = search_params(m->cfg, m->vpad, prompts + (size_t)chunk0 * P, n, K, P, sot_index, o);
+  const SearchParams sp = search_params(m->cfg, m->vpad, n, K, o);
   Step st = choose_step(m, n, K, sp.fake_logits);
-  if (sp.max_steps <= 0) {
+  const int max_steps = o.max_length - P;
+  if (max_steps <= 0) {
     const int num_hyp = std::max(1, o.num_hypotheses);
     for (int b = 0; b < n; ++b)
       for (int h = 0; h < num_hyp; ++h) {
@@ -1357,11 +1400,268 @@ static void generate_group(Model* m, Encoded* e, int chunk0, int n, const int32_
   B2W_CUDA(cudaMemsetAsync(sb.fin_count, 0, n * 4, s));
   B2W_CUDA(cudaMemsetAsync(sb.fin_len, 0xFF, (size_t)n * kMaxFinished * 4, s));
   B2W_CUDA(cudaMemsetAsync(sb.no_speech, 0, n * 4, s));
+  {
+    // the group's first prompt decides the timestamp rules of all of its chunks; item ids are the chunks' indices in the group
+    std::vector<ChunkParams> cps(n);
+    for (int b = 0; b < n; ++b)
+      cps[b] = chunk_params(m->cfg, prompts + (size_t)chunk0 * P, P, sot_index, o.max_length, b, o.return_no_speech_prob);
+    B2W_CUDA(cudaMemcpyAsync(sb.chunk, cps.data(), n * sizeof(ChunkParams), cudaMemcpyHostToDevice, s));
+    B2W_CUDA(cudaStreamSynchronize(s));
+  }
 
   if (!sp.fake_logits && P > 1) prefill(m, e, chunk0, n, prompts, P, K, sot_index, o.return_no_speech_prob);
   bind_step(m, st, e, chunk0, prompts, P, sp);
-  decode_loop(m, st, P, sp.max_steps);
-  collect_hypotheses(m, chunk0, n, K, o, out_ids, out_lens, out_scores, out_ns);
+  decode_loop(m, st, P, max_steps);
+  collect_hypotheses(m, 0, chunk0, n, K, o, out_ids, out_lens, out_scores, out_ns);
+}
+
+// ---- decode session: a fixed set of S slots of K rows, each refilled from a queue as soon as its item finishes ----------------
+// Its decode workspace (self-KV cache, search buffers, slot binding table and step graph) is its own: swapped into the model
+// for the duration of each call, so generate / align / detect_language calls in between do not disturb the slots.
+struct DecodeWorkspace {
+  size_t kv_elems = 0;
+  __half *kcache = nullptr, *vcache = nullptr;
+  SearchBuffers sb{};
+  void* sb_blob = nullptr;
+  int sb_B = 0, sb_K = 0;
+  DecBindings* d_bind = nullptr;
+  DecBindings h_bind{};
+  std::vector<DecBindings> h_binds;
+  SearchParams h_params{};
+  cudaGraphExec_t step_graph = nullptr;
+  int64_t step_graph_kernels = 0;
+  StepGraphKey step_graph_key{};
+};
+
+static void swap_workspace(Model* m, DecodeWorkspace& w) {
+  std::swap(m->kv_elems, w.kv_elems);
+  std::swap(m->kcache, w.kcache);
+  std::swap(m->vcache, w.vcache);
+  std::swap(m->sb, w.sb);
+  std::swap(m->sb_blob, w.sb_blob);
+  std::swap(m->sb_B, w.sb_B);
+  std::swap(m->sb_K, w.sb_K);
+  std::swap(m->d_bind, w.d_bind);
+  std::swap(m->h_bind, w.h_bind);
+  std::swap(m->h_binds, w.h_binds);
+  std::swap(m->h_params, w.h_params);
+  std::swap(m->step_graph, w.step_graph);
+  std::swap(m->step_graph_kernels, w.step_graph_kernels);
+  std::swap(m->step_graph_key, w.step_graph_key);
+  m->sb.suppress = m->d_suppress;
+}
+
+struct ScopedWorkspace {
+  Model* m;
+  DecodeWorkspace& w;
+  ScopedWorkspace(Model* m_, DecodeWorkspace& w_) : m(m_), w(w_) { swap_workspace(m, w); }
+  ~ScopedWorkspace() { swap_workspace(m, w); }
+};
+
+// Drops one reference to an encoder output (under the owner's lock); the last one frees it once the stream has drained.
+static void release_encoded(Model* m, Encoded* e) {
+  if (!e || --e->refs > 0) return;
+  cudaStreamSynchronize(m->stream);
+  delete e;
+}
+
+struct SessionItem {
+  int id;
+  Encoded* e;        // holds a reference
+  int index;         // item of e
+  std::vector<int32_t> prompt;
+  int max_length, sot_index;
+};
+
+struct Session {
+  Model* m;
+  b2w_gen_opts o{};
+  std::vector<int32_t> suppress_ids;  // o.suppress_tokens points here
+  std::vector<uint8_t> mask;
+  SearchParams sp{};
+  int K = 1, S = 1, next_id = 0;
+  DecodeWorkspace ws;
+  std::deque<SessionItem> queue;
+  std::vector<SessionItem> slot;      // slot[b].id < 0: idle
+  std::vector<Encoded*> slot_enc;     // the encoder output slot b is bound to (a reference, kept until the slot is rebound)
+  std::vector<DecBindings> bind;      // the step's slot table
+  SlotReset* d_resets = nullptr;      // [S]
+  int* d_targets = nullptr;           // [kMaxRows]
+  float* d_probs = nullptr;           // [kMaxRows]
+  RowInfo* d_rows_save = nullptr;     // [kMaxRows] the step's rows and input tokens while a forced pass uses the row table
+  int* d_tokens_save = nullptr;       // [kMaxRows]
+  bool started = false;
+  int64_t steps = 0, live_rows = 0;
+  // b2w_session_debug_record: every step's raw logits of each occupied slot (K = 1), kept per item until fetched
+  bool record = false;
+  float* d_rec = nullptr;             // [S][n_ctx][n_vocab]
+  std::vector<int> rec_steps;         // [S] steps recorded since the slot's last refill
+  std::map<int, std::vector<float>> rec_items;
+
+  ~Session() {
+    for (SessionItem& it : queue) release_encoded(m, it.e);
+    for (Encoded* e : slot_enc) release_encoded(m, e);
+    cudaStreamSynchronize(m->stream);
+    for (void* p : {(void*)ws.kcache, (void*)ws.vcache, ws.sb_blob, (void*)ws.d_bind, (void*)d_resets, (void*)d_targets, (void*)d_probs,
+                    (void*)d_rows_save, (void*)d_tokens_save, (void*)d_rec})
+      if (p) cudaFree(p);
+    if (ws.step_graph) cudaGraphExecDestroy(ws.step_graph);
+  }
+};
+
+static void session_bind_slot(Session& ss, int b, Encoded* e, int index) {
+  ++e->refs;
+  release_encoded(ss.m, ss.slot_enc[b]);
+  ss.slot_enc[b] = e;
+  ss.bind[b] = DecBindings{e->xkv, e->B, index};
+}
+
+// Gives every idle slot the next queued item: one reset launch for all of them, then one forced decoding of their prompts[:-1]
+// (shorter prompts padded with their last token: those keys are rewritten by the steps before any row reads them), which also
+// gives the no-speech probability of items whose <|startoftranscript|> is not the last prompt token.  Runs with the session's
+// workspace bound.
+static void session_refill(Session& ss) {
+  Model* m = ss.m;
+  const b2w_config& c = m->cfg;
+  cudaStream_t s = m->stream;
+  if (!ss.started && ss.queue.empty()) return;
+  std::vector<SlotReset> resets;
+  std::vector<int> filled;
+  for (int b = 0; b < ss.S && !ss.queue.empty(); ++b) {
+    if (ss.slot[b].id >= 0) continue;
+    SessionItem it = std::move(ss.queue.front());
+    ss.queue.pop_front();
+    const int P = (int)it.prompt.size();
+    SlotReset r{};
+    r.slot = b;
+    r.last_token = it.prompt[P - 1];
+    r.done = 0;
+    r.cp = chunk_params(c, it.prompt.data(), P, it.sot_index, it.max_length, it.id, ss.o.return_no_speech_prob);
+    resets.push_back(r);
+    filled.push_back(b);
+    if (ss.record) ss.rec_steps[b] = 0;
+    session_bind_slot(ss, b, it.e, it.index);
+    release_encoded(m, it.e);  // the queue's reference; the slot holds its own
+    ss.slot[b] = std::move(it);
+  }
+  if (!ss.started) {  // slots that never had an item idle as done chunks bound to a live encoder output
+    Encoded* any = nullptr;
+    for (int b = 0; b < ss.S && !any; ++b) any = ss.slot_enc[b];
+    for (int b = 0; b < ss.S; ++b) {
+      if (ss.slot_enc[b]) continue;
+      session_bind_slot(ss, b, any, 0);
+      SlotReset r{};
+      r.slot = b;
+      r.last_token = c.sot;
+      r.done = 1;
+      r.cp = ChunkParams{1, 1, 0, 0, 0, {0, 0, 0}};
+      resets.push_back(r);
+    }
+    B2W_CUDA(cudaMemsetAsync(m->sb.state, 0, sizeof(SearchState), s));
+    B2W_CUDA(cudaMemsetAsync(m->sb.done, 0, ss.S * 4, s));
+    ss.started = true;
+  }
+  if (resets.empty()) return;
+  B2W_CUDA(cudaMemcpyAsync(ss.d_resets, resets.data(), resets.size() * sizeof(SlotReset), cudaMemcpyHostToDevice, s));
+  search_reset_slots(ss.d_resets, (int)resets.size(), ss.S, ss.K, m->sb, s);
+  B2W_CUDA(cudaStreamSynchronize(s));
+  if (filled.empty()) return;
+  int n_tok = 0;
+  for (int b : filled) n_tok = std::max(n_tok, (int)ss.slot[b].prompt.size() - 1);
+  if (n_tok > 0) {
+    ScopedStage st(m, B2W_T_PREFILL);
+    const int n = (int)filled.size(), R = ss.S * ss.K;
+    // the forced passes use the row table: the occupied slots' rows and tokens are put back afterwards
+    B2W_CUDA(cudaMemcpyAsync(ss.d_rows_save, m->sb.rows, R * sizeof(RowInfo), cudaMemcpyDeviceToDevice, s));
+    B2W_CUDA(cudaMemcpyAsync(ss.d_tokens_save, m->sb.tokens_in, R * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    ForcedChunks fc{std::vector<DecBindings>(n), filled, ss.S};
+    std::vector<int32_t> toks((size_t)n * n_tok);
+    for (int j = 0; j < n; ++j) {
+      const SessionItem& it = ss.slot[filled[j]];
+      fc.bind[j] = ss.bind[filled[j]];
+      for (int i = 0; i < n_tok; ++i) toks[(size_t)j * n_tok + i] = it.prompt[std::min(i, std::max(0, (int)it.prompt.size() - 2))];
+    }
+    forced_decode(m, fc, toks.data(), n_tok, n_tok, ss.K, false, nullptr, [&](int i0, int i1) {
+      if (!ss.o.return_no_speech_prob) return;
+      const int rpc = i1 - i0;
+      std::vector<int> targets((size_t)n * rpc, -1);
+      std::vector<int> rows_of(n, -1);
+      for (int j = 0; j < n; ++j) {
+        const SessionItem& it = ss.slot[filled[j]];
+        if (it.sot_index >= i0 && it.sot_index < i1 && it.sot_index < (int)it.prompt.size() - 1) {
+          rows_of[j] = j * rpc + it.sot_index - i0;
+          targets[rows_of[j]] = c.no_speech;
+        }
+      }
+      if (std::all_of(rows_of.begin(), rows_of.end(), [](int r) { return r < 0; })) return;
+      logits_gemm(m, n * rpc);
+      B2W_CUDA(cudaMemcpyAsync(ss.d_targets, targets.data(), targets.size() * 4, cudaMemcpyHostToDevice, s));
+      row_target_probs(m->d_logits, m->vpad, n * rpc, c.n_vocab, ss.d_targets, ss.d_probs, s);
+      for (int j = 0; j < n; ++j)
+        if (rows_of[j] >= 0)
+          B2W_CUDA(cudaMemcpyAsync(m->sb.no_speech + filled[j], ss.d_probs + rows_of[j], 4, cudaMemcpyDeviceToDevice, s));
+      B2W_CUDA(cudaStreamSynchronize(s));  // targets goes out of scope
+    });
+    B2W_CUDA(cudaMemcpyAsync(m->sb.rows, ss.d_rows_save, R * sizeof(RowInfo), cudaMemcpyDeviceToDevice, s));
+    B2W_CUDA(cudaMemcpyAsync(m->sb.tokens_in, ss.d_tokens_save, R * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  }
+}
+
+// One b2w_session_run: refill idle slots, then replay the step graph until a polled done[] shows at least one of the occupied
+// slots finished; their results go to the outputs, their slots become idle.  Returns the number of finished items (0 when the
+// queue and the slots are empty).
+static int session_run(Session& ss, int32_t* out_item, int32_t* out_ids, int32_t* out_lens, float* out_scores, float* out_ns) {
+  Model* m = ss.m;
+  ScopedWorkspace bound(m, ss.ws);
+  cudaStream_t s = m->stream;
+  B2W_CUDA(cudaMemcpyAsync(m->d_suppress, ss.mask.data(), m->vpad, cudaMemcpyHostToDevice, s));
+  prepare_decode(m, nullptr, ss.S, ss.K);
+  session_refill(ss);
+  int live = 0;
+  for (const SessionItem& it : ss.slot) live += it.id >= 0;
+  if (live == 0) return 0;
+  Step st = choose_step(m, ss.S, ss.K, false);
+  step_args(m, st);
+  m->h_params = ss.sp;
+  B2W_CUDA(cudaMemcpyAsync(const_cast<SearchParams*>(m->sb.params), &m->h_params, sizeof(SearchParams), cudaMemcpyHostToDevice, s));
+  bind_chunks(m, ss.bind);
+  const int64_t per_step_kernels = step_graph(m, st);
+  const int poll = 4;
+  std::vector<int> fin;
+  {
+    ScopedStage stage(m, B2W_T_DECODE);
+    while (fin.empty()) {
+      for (int i = 0; i < poll; ++i) {
+        B2W_CUDA(cudaGraphLaunch(m->step_graph, s));
+        g_launches += per_step_kernels;
+        const int V = m->cfg.n_vocab, n_ctx = m->cfg.n_text_ctx;
+        for (int b = 0; ss.record && b < ss.S; ++b)
+          if (ss.slot[b].id >= 0 && ss.rec_steps[b] < n_ctx)
+            B2W_CUDA(cudaMemcpyAsync(ss.d_rec + ((size_t)b * n_ctx + ss.rec_steps[b]++) * V, m->d_logits + (size_t)b * m->vpad,
+                                     (size_t)V * 4, cudaMemcpyDeviceToDevice, s));
+      }
+      ss.steps += poll;
+      m->decode_steps += poll;
+      ss.live_rows += (int64_t)poll * live * ss.K;
+      B2W_CUDA(cudaMemcpyAsync(m->h_pinned, m->sb.done, ss.S * sizeof(int), cudaMemcpyDeviceToHost, s));
+      B2W_CUDA(cudaStreamSynchronize(s));
+      for (int b = 0; b < ss.S; ++b)
+        if (ss.slot[b].id >= 0 && m->h_pinned[b]) fin.push_back(b);
+    }
+  }
+  for (size_t j = 0; j < fin.size(); ++j) {
+    const int b = fin[j];
+    collect_hypotheses(m, b, (int)j, 1, ss.K, ss.o, out_ids, out_lens, out_scores, out_ns);
+    out_item[j] = ss.slot[b].id;
+    if (ss.record) {
+      const size_t V = m->cfg.n_vocab;
+      std::vector<float>& rec = ss.rec_items[ss.slot[b].id];
+      rec.resize((size_t)ss.rec_steps[b] * V);
+      B2W_CUDA(cudaMemcpy(rec.data(), ss.d_rec + (size_t)b * m->cfg.n_text_ctx * V, rec.size() * 4, cudaMemcpyDeviceToHost));
+    }
+    ss.slot[b].id = -1;
+  }
+  return (int)fin.size();
 }
 
 // Debug / measurement switches, read once when a model is created (B2W_BSTEP_STOP is read per generate call, in bind_step).
@@ -1394,6 +1694,9 @@ struct b2w_model {
 };
 struct b2w_encoded {
   Encoded* e;
+};
+struct b2w_session {
+  Session s;
 };
 
 // Runs f(m) with calls on the model serialised, its device current and the kernels f launches added to its counter.
@@ -1672,12 +1975,7 @@ int b2w_encoded_to_host(b2w_model* h, const b2w_encoded* e, float* out) {
 void b2w_encoded_free(b2w_encoded* e) {
   if (!e) return;
   if (e->e)  // the owner's stream may still read the output; ~Encoded returns its buffers to the owner's pool
-    guarded([&] {
-      with_model(e->e->owner, [&](Model* m) {
-        cudaStreamSynchronize(m->stream);
-        delete e->e;
-      });
-    });
+    guarded([&] { with_model(e->e->owner, [&](Model* m) { release_encoded(m, e->e); }); });
   delete e;
 }
 
@@ -1704,6 +2002,128 @@ int b2w_generate(b2w_model* h, b2w_encoded* enc, const int32_t* prompts, int32_t
   });
 }
 
+int b2w_session_create(b2w_model* h, const b2w_gen_opts* opts, int32_t* slots, b2w_session** out) {
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(opts && slots && out, "null argument");
+    B2W_CHECK(*slots >= 0, "slots must be 0 (as many as fit) or positive");
+    B2W_CHECK(!opts->debug_fake_logits, "a decode session decodes encoder outputs: debug_fake_logits is not supported");
+    B2W_CHECK(opts->n_suppress_tokens >= 0 && (opts->n_suppress_tokens == 0 || opts->suppress_tokens), "suppress_tokens");
+    const int K = check_gen_opts(m->cfg, *opts);
+    std::unique_ptr<b2w_session> h2(new b2w_session);
+    Session& ss = h2->s;
+    ss.m = m;
+    ss.o = *opts;
+    ss.suppress_ids.assign(opts->suppress_tokens, opts->suppress_tokens + opts->n_suppress_tokens);
+    ss.o.suppress_tokens = ss.suppress_ids.data();
+    ss.mask = suppress_mask(m->cfg, m->vpad, ss.o);
+    ss.K = K;
+    ss.S = std::max(1, kMaxRows / K);
+    if (*slots > 0) ss.S = std::min(ss.S, (int)*slots);
+    ss.sp = search_params(m->cfg, m->vpad, ss.S, K, ss.o);
+    ss.slot.resize(ss.S);
+    for (SessionItem& it : ss.slot) it.id = -1;
+    ss.slot_enc.assign(ss.S, nullptr);
+    ss.bind.resize(ss.S);
+    ss.ws.d_bind = dalloc<DecBindings>(kMaxRows);
+    ss.d_resets = dalloc<SlotReset>(ss.S);
+    ss.d_targets = dalloc<int>(kMaxRows);
+    ss.d_probs = dalloc<float>(kMaxRows);
+    ss.d_rows_save = dalloc<RowInfo>(kMaxRows);
+    ss.d_tokens_save = dalloc<int>(kMaxRows);
+    *slots = ss.S;
+    *out = h2.release();
+  });
+}
+
+int b2w_session_push(b2w_session* sh, b2w_encoded* enc, int32_t item_index, const int32_t* prompt, int32_t prompt_len,
+                     int32_t max_length, int32_t* item_id_out) {
+  return guarded([&] {
+    B2W_CHECK(sh && enc && enc->e && prompt && item_id_out, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model* m) {
+      Encoded* e = enc->e;
+      B2W_CHECK(e->owner == m, "the encoder output belongs to another model");
+      B2W_CHECK(item_index >= 0 && item_index < e->B, "item_index is outside the encoder output");
+      B2W_CHECK(prompt_len >= 1, "empty prompt");
+      B2W_CHECK(max_length > prompt_len && max_length <= ss.o.max_length,
+                "max_length must exceed the prompt length and be at most the session's max_length");
+      const int sot_index = validate_prompts(m->cfg, prompt, 1, prompt_len);
+      ensure_cross_kv(m, e);
+      ++e->refs;
+      ss.queue.push_back(SessionItem{ss.next_id, e, item_index, std::vector<int32_t>(prompt, prompt + prompt_len), max_length, sot_index});
+      *item_id_out = ss.next_id++;
+    });
+  });
+}
+
+int b2w_session_run(b2w_session* sh, int32_t* n_out, int32_t* out_item_ids, int32_t* out_ids, int32_t* out_lens, float* out_scores,
+                    float* out_no_speech) {
+  return guarded([&] {
+    B2W_CHECK(sh && n_out && out_item_ids && out_ids && out_lens && out_scores && out_no_speech, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model*) { *n_out = session_run(ss, out_item_ids, out_ids, out_lens, out_scores, out_no_speech); });
+  });
+}
+
+int b2w_session_pending(b2w_session* sh, int32_t* n_out) {
+  return guarded([&] {
+    B2W_CHECK(sh && n_out, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model*) {
+      int n = (int)ss.queue.size();
+      for (const SessionItem& it : ss.slot) n += it.id >= 0;
+      *n_out = n;
+    });
+  });
+}
+
+int b2w_session_counters(b2w_session* sh, int64_t* steps, int64_t* live_rows) {
+  return guarded([&] {
+    B2W_CHECK(sh && steps && live_rows, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model*) {
+      *steps = ss.steps;
+      *live_rows = ss.live_rows;
+    });
+  });
+}
+
+int b2w_session_debug_record(b2w_session* sh) {
+  return guarded([&] {
+    B2W_CHECK(sh, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model* m) {
+      B2W_CHECK(ss.K == 1, "logits are recorded for one row per slot (beam_size 1, num_hypotheses 1)");
+      B2W_CHECK(!ss.started, "recording starts before the first b2w_session_run");
+      if (!ss.d_rec) ss.d_rec = dalloc<float>((size_t)ss.S * m->cfg.n_text_ctx * m->cfg.n_vocab);
+      ss.rec_steps.assign(ss.S, 0);
+      ss.record = true;
+    });
+  });
+}
+
+int b2w_session_debug_logits(b2w_session* sh, int32_t item_id, float* out, int32_t capacity_steps, int32_t* n_steps_out) {
+  return guarded([&] {
+    B2W_CHECK(sh && n_steps_out && (out || capacity_steps == 0) && capacity_steps >= 0, "null argument");
+    Session& ss = sh->s;
+    with_model(ss.m, [&](Model* m) {
+      auto it = ss.rec_items.find(item_id);
+      B2W_CHECK(it != ss.rec_items.end(), "no recorded logits for this item (recording off, item unfinished or already fetched)");
+      const size_t V = m->cfg.n_vocab, n = it->second.size() / V;
+      B2W_CHECK(n <= (size_t)capacity_steps, "output buffer too small");
+      std::copy(it->second.begin(), it->second.end(), out);
+      *n_steps_out = (int32_t)n;
+      ss.rec_items.erase(it);
+    });
+  });
+}
+
+void b2w_session_destroy(b2w_session* sh) {
+  if (!sh) return;
+  Model* m = sh->s.m;
+  guarded([&] { with_model(m, [&](Model*) { delete sh; }); });
+}
+
 int b2w_detect_language(b2w_model* h, b2w_encoded* enc, float* probs) {
   return guarded(h, [&](Model* m) {
     B2W_CHECK(enc && enc->e && probs, "null argument");
@@ -1716,7 +2136,7 @@ int b2w_detect_language(b2w_model* h, b2w_encoded* enc, float* probs) {
     const std::vector<int32_t> sot(group, m->cfg.sot);
     for (int c0 = 0; c0 < e->B; c0 += group) {
       const int n = std::min(group, e->B - c0);
-      forced_decode(m, e, c0, n, sot.data(), 1, 1, 1, true, nullptr, [&](int, int) {
+      forced_decode(m, forced_range(e, c0, n), sot.data(), 1, 1, 1, true, nullptr, [&](int, int) {
         logits_gemm(m, n);
         lang_probs_from_logits(m->d_logits, m->vpad, n, m->cfg.lang_begin, nl, d_probs + (size_t)c0 * nl, m->stream);
       });
@@ -1843,7 +2263,7 @@ static void align_run(Model* m, const Encoded* e, int chunk0, const int32_t* sta
       std::copy(it.text, it.text + it.n_text, p + n_start + 1);
     }
     const AlignCapture cap{m->d_align_heads, n_heads, d_cap, g.T, g.nf};
-    forced_decode(m, e, chunk0 + g.i0, g.n, toks.data(), g.T, g.T, 1, true, &cap, [&](int i0, int i1) {
+    forced_decode(m, forced_range(e, chunk0 + g.i0, g.n), toks.data(), g.T, g.T, 1, true, &cap, [&](int i0, int i1) {
       const int R = g.n * (i1 - i0);
       const size_t off = g.tp_off + (size_t)g.n * i0;
       logits_gemm(m, R);
@@ -2347,12 +2767,14 @@ int b2w_debug_cross_attn(int32_t device, const uint16_t* q, const uint16_t* kv, 
     const int d = 64 * H, R = n_chunks * rows_per_chunk, T = 1500;
     const size_t groups = (size_t)n_chunks * H * ds_xqgroups(rows_per_chunk);
     ScratchBufs sb;
-    const DecBindings bind{sb.put<__half>(kv, (size_t)2 * n_chunks * H * T * 64), n_chunks, 0};
+    const __half* xkv = sb.put<__half>(kv, (size_t)2 * n_chunks * H * T * 64);
+    std::vector<DecBindings> bind(n_chunks);
+    for (int b = 0; b < n_chunks; ++b) bind[b] = DecBindings{xkv, n_chunks, b};
     DStepArgs a{};
     a.q = sb.put<__half>(q, (size_t)R * d);
     __half* o = sb.alloc<__half>((size_t)R * d);
     a.ao = o;
-    a.bind = sb.put<DecBindings>(&bind, 1);
+    a.bind = sb.put<DecBindings>(bind.data(), bind.size());
     a.xpart = sb.alloc<float>(groups * kDsXSplits * kDsXQ * 66);
     a.xcounters = sb.put<int>(nullptr, 0, groups);
     a.H = H; a.T = T; a.d = d; a.rows_per_chunk = rows_per_chunk; a.n_chunks = n_chunks;
@@ -2374,7 +2796,7 @@ int b2w_debug_logits(b2w_model* h, b2w_encoded* enc, const int32_t* tokens, int3
     std::vector<float> tmp((size_t)kMaxRows * m->vpad);
     for (int c0 = 0; c0 < batch; c0 += group) {
       const int n = std::min(group, batch - c0);
-      forced_decode(m, e, c0, n, tokens + (size_t)c0 * n_tok, n_tok, n_tok, 1, true, nullptr, [&](int i0, int i1) {
+      forced_decode(m, forced_range(e, c0, n), tokens + (size_t)c0 * n_tok, n_tok, n_tok, 1, true, nullptr, [&](int i0, int i1) {
         const int rpc = i1 - i0;
         logits_gemm(m, n * rpc);
         B2W_CUDA(cudaMemcpyAsync(tmp.data(), m->d_logits, (size_t)n * rpc * m->vpad * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -2406,12 +2828,12 @@ int b2w_debug_step_logits(b2w_model* h, b2w_encoded* enc, const int32_t* prompts
     prepare_decode(m, e, n, K);
     cudaStream_t s = m->stream;
     const SearchBuffers& sb = m->sb;
-    forced_decode(m, e, 0, n, prompts, P, P - 1, K, true, nullptr, [](int, int) {});  // the prompt's keys, as prefill writes them
+    forced_decode(m, forced_range(e, 0, n), prompts, P, P - 1, K, true, nullptr, [](int, int) {});  // the prompt's keys, as prefill writes them
     b2w_gen_opts o;
     b2w_gen_opts_default(&o);
     o.beam_size = K;
     o.max_length = P + n_steps;
-    bind_step(m, st, e, 0, prompts, P, search_params(c, m->vpad, prompts, n, K, P, -1, o));
+    bind_step(m, st, e, 0, prompts, P, search_params(c, m->vpad, n, K, o));
     // anc[r][j]: the slot that holds key j of row r.  Keys of the prompt sit in slot 0; relinked as search_update does.
     std::vector<uint8_t> anc((size_t)R * n_ctx, 0), prev;
     std::vector<RowInfo> rows(R);
@@ -2463,9 +2885,9 @@ int b2w_debug_search(int32_t device, b2w_search_desc* d) {
     B2W_CHECK(P >= 1 && P <= n_ctx, "prompt length");
     const int sot_index = validate_prompts(c, d->prompt, 1, P);
     B2W_CHECK(t >= 0 && t < o.max_length - P, "step must be one a generate call with max_length runs");
-    std::vector<int32_t> prompts((size_t)n * P);
-    for (int b = 0; b < n; ++b) std::copy(d->prompt, d->prompt + P, prompts.begin() + (size_t)b * P);
-    const SearchParams sp = search_params(c, vpad, prompts.data(), n, K, P, sot_index, o);
+    const SearchParams sp = search_params(c, vpad, n, K, o);
+    std::vector<ChunkParams> cps(n);
+    for (int b = 0; b < n; ++b) cps[b] = chunk_params(c, d->prompt, P, sot_index, o.max_length, b, o.return_no_speech_prob);
     const bool beam = sp.mode == 0;
     for (size_t i = 0; i < (size_t)R * t; ++i) B2W_CHECK(d->hist[i] >= 0 && d->hist[i] < V, "history token id out of range");
     for (size_t i = 0; i < (size_t)R * (P - 1 + t); ++i) B2W_CHECK(d->anc[i] < K, "ancestry slot out of range");
@@ -2488,6 +2910,7 @@ int b2w_debug_search(int32_t device, b2w_search_desc* d) {
     SearchState state{t, d->n_done, cur, 0};
     sb.state = hb.put<SearchState>(&state, 1);
     sb.params = hb.put<SearchParams>(&sp, 1);
+    sb.chunk = hb.put<ChunkParams>(cps.data(), n);
     std::vector<RowInfo> rows(R);
     for (int r = 0; r < R; ++r) rows[r] = RowInfo{r / K, r % K, pos, 0};
     sb.rows = hb.put<RowInfo>(rows.data(), R);

@@ -51,6 +51,7 @@ struct Encoded {
   size_t enc_bytes = 0, xkv_bytes = 0;
   __half* enc_out = nullptr;  // [B][1500][d] fp16
   __half* xkv = nullptr;      // lazily: [L][2][B][H][T][64] fp16
+  int refs = 1;               // the b2w_encoded handle, and one per decode-session slot or queued item that reads it
   ~Encoded();
 };
 
@@ -137,7 +138,8 @@ struct Model {
   float *d_stats = nullptr, *d_gpart = nullptr, *d_stpart = nullptr;
   __half *d_h16 = nullptr, *d_xn16 = nullptr;
   std::optional<StepPath> forced_step;  // B2W_STEP=dstep|bstep|layers (tests and tools)
-  DecBindings h_bind{};
+  DecBindings h_bind{};                // chunk 0's entry of the last bound table
+  std::vector<DecBindings> h_binds;    // host copy of d_bind's entries
   SearchParams h_params{};
   // search buffers
   SearchBuffers sb{};

@@ -83,14 +83,16 @@ __global__ void __launch_bounds__(kRowThreads) search_rows_kernel(const float* _
   const int b = r / p.K, k = r % p.K;
   const int V = p.n_vocab;
   const RowInfo ri = bf.rows[r];
-  const int step = ri.pos - (p.prompt_len - 1);
+  const ChunkParams cp = bf.chunk[b];
+  const int step = ri.pos - (cp.prompt_len - 1);
+  const int noise_row = cp.item * p.K + k;  // the item's own row index: its draws do not depend on the slot it occupies
   const int cur = ri.pos & 1;  // history double buffer is indexed by the parity of the absolute position
   const int* hist = bf.hist + ((long long)cur * p.B * p.K + r) * bf.n_ctx;
   const int len = step;  // tokens generated so far by this row
   const float* row = logits + (long long)r * p.vpad;
 
   // ---- no_speech probability from the raw first-step logits (sot is the last prompt token) ----
-  if (p.want_no_speech_first && step == 0 && k == 0) {
+  if (cp.ns_first && step == 0 && k == 0) {
     float mx = -INFINITY;
 #pragma unroll 4
     for (int v = tid; v < V; v += kRowThreads) mx = fmaxf(mx, row[v]);
@@ -171,7 +173,7 @@ __global__ void __launch_bounds__(kRowThreads) search_rows_kernel(const float* _
   __syncthreads();
 
   // ---- Whisper timestamp rules ----
-  if (p.timestamp_rules) {
+  if (cp.timestamp_rules) {
     const int ts0 = p.timestamp_begin;
     if (tid == 0) {
       s[p.no_timestamps] = B2W_LOWEST;
@@ -263,7 +265,7 @@ __global__ void __launch_bounds__(kRowThreads) search_rows_kernel(const float* _
       x = sampling ? -INFINITY : (x - lse);  // CT2 keeps "lowest" (finite) scores for masked ids in beam search
     } else {
       x = x - lse;
-      if (sampling) x = x * inv_t + gumbel_u32(p.seed, r, step, v);
+      if (sampling) x = x * inv_t + gumbel_u32(p.seed, noise_row, step, v);
     }
     s[v] = x;
   }
@@ -319,7 +321,7 @@ __global__ void __launch_bounds__(kRowThreads) search_rows_kernel(const float* _
         float sc;
         if (sampling) {
           // score of a draw: tempered log-prob (what CTranslate2's RandomSampler gathers)
-          sc = (best.i == 0x7fffffff) ? B2W_LOWEST : (best.v - gumbel_u32(p.seed, r, step, best.i));
+          sc = (best.i == 0x7fffffff) ? B2W_LOWEST : (best.v - gumbel_u32(p.seed, noise_row, step, best.i));
         } else {
           sc = best.v;
         }
@@ -356,10 +358,11 @@ __global__ void __launch_bounds__(128) search_update_kernel(const SearchBuffers 
   const int b = blockIdx.x, tid = threadIdx.x;
   const int K = p.K, V = p.n_vocab, n_ctx = bf.n_ctx, ncand = p.ncand;
   const int r0 = b * K;
+  const ChunkParams cp = bf.chunk[b];
   const int pos = bf.rows[r0].pos;
-  const int step = pos - (p.prompt_len - 1);
+  const int step = pos - (cp.prompt_len - 1);
   const int cur = pos & 1, nxt = cur ^ 1;
-  const bool is_last = (step + 1 >= p.max_steps);
+  const bool is_last = (step + 1 >= cp.max_steps);
   const long long RB = (long long)p.B * K;
   for (int i = tid; i < K * ncand; i += blockDim.x) {
     const int k = i / ncand, c = i - k * ncand;
@@ -502,7 +505,8 @@ __global__ void __launch_bounds__(128) search_update_kernel(const SearchBuffers 
       ad[pos] = (uint8_t)pk;
       bf.cum[(long long)nxt * RB + r0 + k] = newcum[k];
       bf.tokens_in[r0 + k] = newtok[k];
-      bf.rows[r0 + k].pos = pos + 1;
+      // a generate call ends by max_length <= n_ctx; a finished slot of a decode session idles at the last position until reset
+      bf.rows[r0 + k].pos = min(pos + 1, n_ctx - 1);
     }
   }
 }
@@ -512,13 +516,48 @@ void search_update(int B, const SearchBuffers& b, cudaStream_t s) {
   B2W_LAUNCHED();
 }
 
+// One CTA per reset slot: clears everything search_rows / search_update keep for the slot (cumulative scores, history and
+// KV ancestry of its rows in both buffers, finished hypotheses, done flag and its share of n_done, no-speech probability),
+// installs the occupant's chunk parameters and starts its rows at the last prompt position.  Other slots are not touched.
+__global__ void __launch_bounds__(256) search_reset_kernel(const SlotReset* __restrict__ resets, int B, int K, const SearchBuffers bf) {
+  const SlotReset rs = resets[blockIdx.x];
+  const int b = rs.slot, tid = threadIdx.x, n_ctx = bf.n_ctx;
+  const long long RB = (long long)B * K;
+  for (int buf = 0; buf < 2; ++buf)
+    for (int k = 0; k < K; ++k) {
+      const long long row = buf * RB + (long long)b * K + k;
+      for (int i = tid; i < n_ctx; i += blockDim.x) {
+        bf.hist[row * n_ctx + i] = 0;
+        bf.anc[row * n_ctx + i] = 0;
+      }
+      if (tid == 0) bf.cum[row] = 0.f;
+    }
+  for (int i = tid; i < kMaxFinished; i += blockDim.x) bf.fin_len[b * kMaxFinished + i] = -1;
+  if (tid < K) {
+    bf.rows[b * K + tid] = RowInfo{b, tid, rs.cp.prompt_len - 1, 0};
+    bf.tokens_in[b * K + tid] = rs.last_token;
+  }
+  if (tid == 0) {
+    bf.chunk[b] = rs.cp;
+    bf.fin_count[b] = 0;
+    bf.no_speech[b] = 0.f;
+    const int was = bf.done[b];
+    bf.done[b] = rs.done;
+    if (was != rs.done) atomicAdd(&bf.state->n_done, rs.done - was);
+  }
+}
+void search_reset_slots(const SlotReset* resets, int n, int B, int K, const SearchBuffers& b, cudaStream_t s) {
+  search_reset_kernel<<<n, 256, 0, s>>>(resets, B, K, b);
+  B2W_LAUNCHED();
+}
+
 // ---- deterministic stand-in for the decoder (tests of the search logic only) -------------------------------------------
 // logits[r][v] = u24(hash(token_in, step, v)) * 2^-20 - 8  (+3 for timestamps, +0.25*step for EOT); mirrored in
 // tests/test_search.py so the device search can be compared bit-for-bit with the oracle's search.
 __global__ void fake_logits_kernel(float* __restrict__ logits, const SearchBuffers bf) {
   const SearchParams p = *bf.params;
   const int r = blockIdx.y;
-  const int step = bf.rows[r].pos - (p.prompt_len - 1);
+  const int step = bf.rows[r].pos - (bf.chunk[r / p.K].prompt_len - 1);
   const unsigned tok = (unsigned)bf.tokens_in[r];
   for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < p.n_vocab; v += gridDim.x * blockDim.x) {
     unsigned h = tok * 0x9E3779B1u ^ ((unsigned)step * 0x85EBCA77u) ^ ((unsigned)v * 0xC2B2AE3Du);
@@ -580,11 +619,12 @@ void row_target_probs(const float* logits, int row_stride, int R, int n_vocab, c
 
 // Cross-attention probabilities of the alignment heads of one layer for forced-decoding rows (Whisper.align): CTA per
 // (alignment head, row); softmax over all T encoder positions, the first nf written out as out[chunk][head][pos][t] for the
-// row's chunk (relative to bind->chunk0) and position.  K rows are stored with their 16-byte chunks at chunk ^ (t & 7)
+// row's pass chunk (r / rows_per_chunk, the index ds_cross_attn_kernel uses too) and position, against bind[chunk].  K rows are stored with their 16-byte chunks at chunk ^ (t & 7)
 // (gemm.cu EPI_F16_XKV).
 __global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restrict__ q, const DecBindings* __restrict__ bind,
                                                           const RowInfo* __restrict__ rows, int layer, const int2* __restrict__ heads,
-                                                          float* __restrict__ out, int n_tok, int nf, int H, int T, int d) {
+                                                          float* __restrict__ out, int n_tok, int nf, int rows_per_chunk, int H, int T,
+                                                          int d) {
   const int2 lh = heads[blockIdx.x];
   if (lh.x != layer) return;
   __shared__ float qs[64];
@@ -592,9 +632,10 @@ __global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restri
   __shared__ float red[32];
   const int r = blockIdx.y, h = lh.y, tid = threadIdx.x;
   const RowInfo ri = rows[r];
-  const DecBindings bd = *bind;
+  const int chunk = r / rows_per_chunk;
+  const DecBindings bd = bind[chunk];
   const long long per = (long long)bd.B_total * H * T * 64;
-  const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + (((long long)(bd.chunk0 + ri.chunk) * H + h) * T) * 64;
+  const __half* Kb = bd.xkv + ((long long)layer * 2 + 0) * per + (((long long)bd.item * H + h) * T) * 64;
   if (tid < 64) qs[tid] = __half2float(q[(long long)r * d + h * 64 + tid]) * 0.125f;
   __syncthreads();
   float mx = -INFINITY;
@@ -621,13 +662,13 @@ __global__ void __launch_bounds__(256) align_probs_kernel(const __half* __restri
     sm += e;
   }
   sm = block_sum(sm, red);
-  float* o = out + (((long long)ri.chunk * gridDim.x + blockIdx.x) * n_tok + ri.pos) * nf;
+  float* o = out + (((long long)chunk * gridDim.x + blockIdx.x) * n_tok + ri.pos) * nf;
   for (int t = tid; t < nf; t += 256) o[t] = sc[t] / sm;
 }
 void align_probs(const __half* q, const DecBindings* bind, const RowInfo* rows, int layer, const int2* heads, int n_heads, float* out,
-                 int n_tok, int nf, int R, int H, int T, int d, cudaStream_t s) {
+                 int n_tok, int nf, int R, int rows_per_chunk, int H, int T, int d, cudaStream_t s) {
   B2W_CHECK(T <= 1536, "align_probs: encoder length");
-  align_probs_kernel<<<dim3(n_heads, R), 256, 0, s>>>(q, bind, rows, layer, heads, out, n_tok, nf, H, T, d);
+  align_probs_kernel<<<dim3(n_heads, R), 256, 0, s>>>(q, bind, rows, layer, heads, out, n_tok, nf, rows_per_chunk, H, T, d);
   B2W_LAUNCHED();
 }
 

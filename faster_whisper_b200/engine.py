@@ -147,6 +147,8 @@ ABI_SYMBOLS = (
     "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
     "b2w_debug_step_logits", "b2w_debug_self_attn", "b2w_debug_cross_attn", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
+    "b2w_session_create", "b2w_session_push", "b2w_session_run", "b2w_session_pending", "b2w_session_counters", "b2w_session_destroy",
+    "b2w_session_debug_record", "b2w_session_debug_logits",
 )
 
 
@@ -223,6 +225,15 @@ def load_library():
                                             C.c_int64]
         lib.b2w_vad_set_block.argtypes = [C.c_void_p, C.c_int64]
         lib.b2w_vad_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        lib.b2w_session_create.argtypes = [C.c_void_p, C.POINTER(_GenOpts), C.POINTER(C.c_int32), C.POINTER(C.c_void_p)]
+        lib.b2w_session_push.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
+        lib.b2w_session_run.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.b2w_session_pending.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+        lib.b2w_session_counters.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        lib.b2w_session_debug_record.argtypes = [C.c_void_p]
+        lib.b2w_session_debug_logits.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
+        lib.b2w_session_destroy.argtypes = [C.c_void_p]
+        lib.b2w_session_destroy.restype = None
         if lib.b2w_abi_version() != 1:
             raise RuntimeError("libb200whisper ABI version mismatch")
         _lib = lib
@@ -584,6 +595,23 @@ class Whisper:
                 no_speech_prob=float(nsp[b]) if return_no_speech_prob else 0.0))
         return out
 
+    def decode_queue(self, *, beam_size: int = 5, patience: float = 1, num_hypotheses: int = 1, length_penalty: float = 1,
+                     repetition_penalty: float = 1, no_repeat_ngram_size: int = 0, max_length: int = 448, return_scores: bool = False,
+                     return_no_speech_prob: bool = False, max_initial_timestamp_index: int = 50, suppress_blank: bool = True,
+                     suppress_tokens: Optional[Sequence[int]] = (-1,), sampling_topk: int = 1, sampling_temperature: float = 1,
+                     seed: int = 0, slots: int = 0, replica: int = 0) -> "DecodeQueue":
+        """A continuous-batching decoder with ``generate``'s options: ``push`` items, iterate ``(item_id, WhisperGenerationResult)``
+        in completion order.  A finished item's rows take the next queued item instead of idling until a whole batch ends.
+        ``slots``: chunks decoded at once (0: as many as one decode step takes, 80 // rows per chunk)."""
+        rep = self._replicas[replica]
+        o, sup_arr = _gen_opts(rep._lib, self.dims.n_text_ctx, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
+                               length_penalty=length_penalty, repetition_penalty=repetition_penalty,
+                               no_repeat_ngram_size=no_repeat_ngram_size, max_length=max_length, return_scores=return_scores,
+                               return_no_speech_prob=return_no_speech_prob, max_initial_timestamp_index=max_initial_timestamp_index,
+                               suppress_blank=suppress_blank, suppress_tokens=suppress_tokens, sampling_topk=sampling_topk,
+                               sampling_temperature=sampling_temperature, seed=seed)
+        return DecodeQueue(self, rep, o, sup_arr, slots)
+
     # ---- detect_language (transcribe.py:215,1193,1823) ----
     def detect_language(self, features: Union[StorageView, np.ndarray]) -> List[List[Tuple[str, float]]]:
         from .config import LANGUAGE_CODES
@@ -710,6 +738,132 @@ class Whisper:
         with rep.lock:
             _check(rep._lib.b2w_debug_fetch(rep.handle, int(which), _ptr(out), int(n)))
         return out
+
+
+def check_queue_items(prompts, max_lengths, n_vocab: int, sot: int, max_length: int) -> List[Tuple[np.ndarray, int]]:
+    """The checks b2w_session_push makes, over every item before any is queued, so a rejected push queues nothing."""
+    if len(max_lengths) != len(prompts):
+        raise ValueError("one max_length per prompt is required")
+    items = []
+    for p, ml in zip(prompts, max_lengths):
+        pr = np.ascontiguousarray(np.asarray(list(map(int, p)), dtype=np.int32))
+        if pr.size == 0:
+            raise ValueError("empty prompt")
+        if pr.min() < 0 or pr.max() >= n_vocab:
+            raise ValueError("prompt token id out of range")
+        if sot not in pr:
+            raise ValueError("<|startoftranscript|> token was not found in the prompt")
+        if not (pr.size < int(ml) <= max_length):
+            raise ValueError("max_length must exceed the prompt length and be at most the session's max_length")
+        items.append((pr, int(ml)))
+    return items
+
+
+class DecodeQueue:
+    """A native decode session (``Whisper.decode_queue``).  Items are decoded in a fixed set of slots; ``push`` queues them,
+    iteration yields ``(item_id, WhisperGenerationResult)`` as they finish (ids count pushes from 0).  Each pushed encoder output
+    is kept alive on the device until the session no longer reads it."""
+
+    def __init__(self, owner: "Whisper", rep: _Replica, opts: _GenOpts, sup_arr: np.ndarray, slots: int = 0):
+        self._owner, self._rep, self._opts, self._sup = owner, rep, opts, sup_arr
+        self._return_scores = bool(opts.return_scores)
+        self._return_ns = bool(opts.return_no_speech_prob)
+        h, slots = C.c_void_p(), C.c_int32(int(slots))
+        with rep.lock:
+            _check(rep._lib.b2w_session_create(rep.handle, C.byref(opts), C.byref(slots), C.byref(h)))
+        self._h = h
+        self.slots = int(slots.value)
+        H, L = max(1, opts.num_hypotheses), opts.max_length
+        self._ids = np.zeros((self.slots, H, L), np.int32)
+        self._lens = np.zeros((self.slots, H), np.int32)
+        self._scores = np.zeros((self.slots, H), np.float32)
+        self._ns = np.zeros((self.slots,), np.float32)
+        self._items = np.zeros((self.slots,), np.int32)
+
+    def push(self, storage_view: StorageView, prompts: Sequence[Sequence[int]], max_lengths: Optional[Sequence[int]] = None) -> List[int]:
+        """Queues item i of ``storage_view`` (a device encoder output of this model) with ``prompts[i]`` (lengths may differ)
+        and ``max_lengths[i]`` (default: the queue's ``max_length``).  Returns the items' ids."""
+        if not isinstance(storage_view, StorageView) or storage_view._handle is None:
+            raise ValueError("push takes a device encoder output (a StorageView from encode / encode_audio)")
+        if self._owner._replica_for(storage_view) is not self._rep:
+            raise ValueError("the encoder output belongs to another replica")
+        if len(prompts) != storage_view.shape[0]:
+            raise ValueError("the number of prompts must match the batch size of the encoder output")
+        if max_lengths is None:
+            max_lengths = [self._opts.max_length] * len(prompts)
+        items = check_queue_items(prompts, max_lengths, self._owner.dims.n_vocab, self._owner.tokens.sot, self._opts.max_length)
+        ids = []
+        for i, (pr, ml) in enumerate(items):
+            out = C.c_int32()
+            with self._rep.lock:
+                _check(self._rep._lib.b2w_session_push(self._handle(), storage_view._handle, i, _ptr(pr), pr.shape[0], int(ml), C.byref(out)))
+            ids.append(int(out.value))
+        return ids
+
+    def _handle(self):
+        if not self._h:
+            raise RuntimeError("the decode queue is closed")
+        return self._h
+
+    def debug_record(self):
+        """Test hook: record every step's raw logits of each occupied slot (one row per slot only); call before the first run."""
+        with self._rep.lock:
+            _check(self._rep._lib.b2w_session_debug_record(self._handle()))
+
+    def debug_logits(self, item_id: int) -> np.ndarray:
+        """[steps][n_vocab] logits recorded for a finished item, from its first step (the last ones may be idle steps)."""
+        cap = self._owner.dims.n_text_ctx
+        out = np.zeros((cap, self._owner.dims.n_vocab), np.float32)
+        n = C.c_int32()
+        with self._rep.lock:
+            _check(self._rep._lib.b2w_session_debug_logits(self._handle(), int(item_id), _ptr(out), cap, C.byref(n)))
+        return out[: n.value]
+
+    def pending(self) -> int:
+        n = C.c_int32()
+        with self._rep.lock:
+            _check(self._rep._lib.b2w_session_pending(self._handle(), C.byref(n)))
+        return int(n.value)
+
+    def counters(self) -> Tuple[int, int]:
+        """(decode steps run, rows of occupied slots summed over the steps)."""
+        st, rows = C.c_int64(), C.c_int64()
+        with self._rep.lock:
+            _check(self._rep._lib.b2w_session_counters(self._handle(), C.byref(st), C.byref(rows)))
+        return int(st.value), int(rows.value)
+
+    def run(self) -> List[Tuple[int, WhisperGenerationResult]]:
+        """Decodes until at least one item finishes; [] when nothing is queued or decoding."""
+        n = C.c_int32()
+        with self._rep.lock:
+            _check(self._rep._lib.b2w_session_run(self._handle(), C.byref(n), _ptr(self._items), _ptr(self._ids), _ptr(self._lens),
+                                                  _ptr(self._scores), _ptr(self._ns)))
+        out = []
+        for j in range(n.value):
+            H = self._lens.shape[1]
+            out.append((int(self._items[j]), WhisperGenerationResult(
+                sequences_ids=[self._ids[j, h, : self._lens[j, h]].tolist() for h in range(H)],
+                scores=[float(x) for x in self._scores[j]] if self._return_scores else [],
+                no_speech_prob=float(self._ns[j]) if self._return_ns else 0.0)))
+        return out
+
+    def __iter__(self):
+        while True:
+            done = self.run()
+            if not done:
+                return
+            yield from done
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h and self._rep._h:  # the session must go before its model; after unload_model its buffers go with the device context
+            self._rep._lib.b2w_session_destroy(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
 
 
 class SileroVad:

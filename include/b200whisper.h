@@ -123,6 +123,36 @@ int b2w_generate(b2w_model* m, b2w_encoded* e, const int32_t* prompts, int32_t p
                  float* out_no_speech);
 void b2w_gen_opts_default(b2w_gen_opts* o);
 
+/* ---- decode session (continuous batching) ------------------------------------------------------
+ * A fixed set of slots (up to 80 / K chunks of K = beam_size, or num_hypotheses when beam_size is 1, rows) decoding
+ * with one set of generate options; a slot whose item finishes takes the next queued item at the next poll.
+ *   b2w_session_create : *slots: 0 for as many slots as a step takes, else at most that many; receives the number of
+ *                        slots (the most items one b2w_session_run returns).
+ *                        The session must be destroyed before its model.
+ *   b2w_session_push   : queues item item_index of e with its own prompt (any length, <|startoftranscript|> anywhere) and
+ *                        max_length (prompt_len < max_length <= opts->max_length); item_id_out receives its id (0, 1, ... in
+ *                        push order), which also keys its sampling noise.  The session keeps e alive while it reads it.
+ *   b2w_session_run    : decodes until at least one item finishes, or returns n_out = 0 when the queue and the slots are
+ *                        empty.  Outputs j < n_out: out_item_ids[j]; out_ids [slots][num_hypotheses][opts->max_length],
+ *                        out_lens / out_scores [slots][num_hypotheses], out_no_speech [slots], as b2w_generate.
+ *   b2w_session_pending: queued plus decoding items.
+ *   b2w_session_counters: decode steps run, and rows of occupied slots summed over them (a slot counts until the poll, every
+ *                        4 steps, that sees it finish: at most 3 steps past its item's last).
+ *   b2w_session_debug_record / b2w_session_debug_logits (tests): for a session with one row per slot, record every step's raw
+ *                        logits of each occupied slot; fetch an item's [n_steps][n_vocab] once it has finished (steps from its
+ *                        first; the last steps may be idle steps after it finished). */
+typedef struct b2w_session b2w_session;
+int b2w_session_create(b2w_model* m, const b2w_gen_opts* opts, int32_t* slots, b2w_session** out);
+int b2w_session_push(b2w_session* s, b2w_encoded* e, int32_t item_index, const int32_t* prompt, int32_t prompt_len,
+                     int32_t max_length, int32_t* item_id_out);
+int b2w_session_run(b2w_session* s, int32_t* n_out, int32_t* out_item_ids, int32_t* out_ids, int32_t* out_lens,
+                    float* out_scores, float* out_no_speech);
+int b2w_session_pending(b2w_session* s, int32_t* n_out);
+int b2w_session_counters(b2w_session* s, int64_t* steps, int64_t* live_rows);
+int b2w_session_debug_record(b2w_session* s);
+int b2w_session_debug_logits(b2w_session* s, int32_t item_id, float* out, int32_t capacity_steps, int32_t* n_steps_out);
+void b2w_session_destroy(b2w_session* s);
+
 /* Whisper.detect_language(encoder_output) (transcribe.py:215,1193,1823): probs [batch, num_languages]
  * over the language tokens (softmax restricted to them), id order. */
 int b2w_detect_language(b2w_model* m, b2w_encoded* e, float* probs);
