@@ -133,19 +133,34 @@ void* Model::pool_get(size_t bytes) {
   }
   return p;
 }
+// At most 24 GiB and kPoolBuffers buffers stay parked; past either, the oldest are freed.  The count covers a continuous-batching
+// pipeline at any slot count: two buffers per chunk encoder output, fewer than 3 x kMaxRows chunks alive, plus a batch's two and an
+// alignment's scratch.  The byte limit covers it at 16 slots x beam 5 on large-v3 (fewer than 48 chunks, 12 GB), so its steady state
+// never reaches cudaFree there; with more slots at that size a drop in live outputs frees the oldest buffers past 24 GiB.
+constexpr size_t kPoolBuffers = 2 * 3 * kMaxRows + 16;
 void Model::pool_put(void* p, size_t bytes) {
   if (!p) return;
-  if (pool_bytes + bytes > (size_t)24 << 30 || pool.size() >= 16) {
-    cudaFree(p);
-    return;
-  }
   pool.emplace_back(bytes, p);
   pool_bytes += bytes;
+  while (pool_bytes > ((size_t)24 << 30) || pool.size() > kPoolBuffers) {
+    cudaFree(pool.front().second);
+    pool_bytes -= pool.front().first;
+    pool.erase(pool.begin());
+  }
+}
+
+// An encoder-output buffer from the pool, counted in encoded_bytes until ~Encoded returns it.
+static __half* encoded_alloc(Model* m, size_t bytes) {
+  __half* p = reinterpret_cast<__half*>(m->pool_get(bytes));
+  m->encoded_bytes += bytes;
+  return p;
 }
 
 Encoded::~Encoded() {
   if (!owner) return;
   cudaSetDevice(owner->device);
+  if (enc_out) owner->encoded_bytes -= enc_bytes;
+  if (xkv) owner->encoded_bytes -= xkv_bytes;
   owner->pool_put(enc_out, enc_bytes);
   owner->pool_put(xkv, xkv_bytes);
 }
@@ -725,7 +740,7 @@ static std::unique_ptr<Encoded> encode(Model* m, int B, F&& fill) {
   e->B = B;
   const size_t d = m->cfg.n_audio_state;
   e->enc_bytes = (size_t)B * 1500 * d * sizeof(__half);
-  e->enc_out = reinterpret_cast<__half*>(m->pool_get(e->enc_bytes));
+  e->enc_out = encoded_alloc(m, e->enc_bytes);
   for (int b0 = 0; b0 < B; b0 += kEncSub) {
     const int b = std::min(kEncSub, B - b0);
     ensure_encoder_ws(m, std::min(kEncSub, B));
@@ -830,7 +845,7 @@ static void ensure_cross_kv(Model* m, Encoded* e) {
   if (e->xkv) return;
   const int d = m->cfg.n_audio_state, dt = m->cfg.n_text_state, L = m->cfg.n_text_layer, H = m->cfg.n_text_head;
   e->xkv_bytes = (size_t)L * 2 * e->B * 1500 * dt * sizeof(__half);
-  e->xkv = reinterpret_cast<__half*>(m->pool_get(e->xkv_bytes));
+  e->xkv = encoded_alloc(m, e->xkv_bytes);
   ScopedStage st(m, B2W_T_CROSSKV);
   GemmArgs a;
   a.A = e->enc_out;
@@ -2163,13 +2178,15 @@ static void check_align_sequence(const b2w_config& c, const int32_t* start, int 
 }
 
 struct AlignItem {
+  Encoded* e;               // the item's encoder output, and its index there
+  int index;
   const int32_t* text;
   int n_text, nf;
   float* probs;             // host [n_text]: probability of each text token at the position that predicts it
   std::vector<int2> pairs;  // the DTW path (text index, frame index); none when n_text = 0
 };
 
-// Aligns items[k] against chunk chunk0 + k of `e` (arguments already checked).  Consecutive items form groups whose padded
+// Aligns each of `items` against its own encoder item (arguments already checked).  Consecutive items form groups whose padded
 // sequences fit one pass of kMaxRows rows, so that every pass reads each chunk's cross-attention K/V once: splitting a long
 // sequence over the passes of a group would re-read every chunk's K/V in each pass, which costs more than the weights it shares
 // (an item longer than a pass is a group of its own).  The group's cross-attention counters and capture must fit too.  A group's
@@ -2177,7 +2194,7 @@ struct AlignItem {
 // (attention is causal, so they do not change the real rows).  Per group: the forced decode with the capture and the text-token
 // probabilities, then the cost matrix and the DTW on the device.  Pairs, counts and probabilities come back with one copy each
 // and one synchronise.
-static void align_run(Model* m, const Encoded* e, int chunk0, const int32_t* start, int n_start, std::vector<AlignItem>& items, int width) {
+static void align_run(Model* m, const int32_t* start, int n_start, std::vector<AlignItem>& items, int width) {
   const b2w_config& c = m->cfg;
   cudaStream_t s = m->stream;
   const int n_heads = (int)m->align_heads.size(), n_items = (int)items.size();
@@ -2221,7 +2238,8 @@ static void align_run(Model* m, const Encoded* e, int chunk0, const int32_t* sta
     }
   int max_n = 0;
   for (const Group& g : groups) max_n = std::max(max_n, g.n);
-  prepare_decode(m, const_cast<Encoded*>(e), max_n, 1);
+  prepare_decode(m, nullptr, max_n, 1);
+  for (const AlignItem& it : items) ensure_cross_kv(m, it.e);
   if (!m->d_align_heads) {
     m->d_align_heads = dalloc<int2>(n_heads);
     B2W_CUDA(cudaMemcpy(m->d_align_heads, m->align_heads.data(), n_heads * sizeof(int2), cudaMemcpyHostToDevice));
@@ -2263,7 +2281,13 @@ static void align_run(Model* m, const Encoded* e, int chunk0, const int32_t* sta
       std::copy(it.text, it.text + it.n_text, p + n_start + 1);
     }
     const AlignCapture cap{m->d_align_heads, n_heads, d_cap, g.T, g.nf};
-    forced_decode(m, forced_range(e, chunk0 + g.i0, g.n), toks.data(), g.T, g.T, 1, true, &cap, [&](int i0, int i1) {
+    ForcedChunks fc{std::vector<DecBindings>(g.n), std::vector<int>(g.n), g.n};
+    for (int b = 0; b < g.n; ++b) {
+      const AlignItem& it = items[g.i0 + b];
+      fc.bind[b] = DecBindings{it.e->xkv, it.e->B, it.index};
+      fc.kv_chunk[b] = b;
+    }
+    forced_decode(m, fc, toks.data(), g.T, g.T, 1, true, &cap, [&](int i0, int i1) {
       const int R = g.n * (i1 - i0);
       const size_t off = g.tp_off + (size_t)g.n * i0;
       logits_gemm(m, R);
@@ -2321,8 +2345,8 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
     if (n_text == 0) return;
     B2W_CHECK(text_tokens && text_token_probs_out && (alignments_out || capacity_pairs == 0), "bad arguments");
     check_align_sequence(m->cfg, start_sequence, n_start, text_tokens, n_text);
-    std::vector<AlignItem> items{AlignItem{text_tokens, n_text, align_frames(num_frames), text_token_probs_out, {}}};
-    align_run(m, e, batch_index, start_sequence, n_start, items, median_filter_width);
+    std::vector<AlignItem> items{AlignItem{e, batch_index, text_tokens, n_text, align_frames(num_frames), text_token_probs_out, {}}};
+    align_run(m, start_sequence, n_start, items, median_filter_width);
     const std::vector<int2>& p = items[0].pairs;
     *n_pairs_out = (int32_t)p.size();
     if ((int)p.size() > capacity_pairs) throw Error("align: alignment buffer too small", true);
@@ -2333,13 +2357,14 @@ int b2w_align(b2w_model* h, b2w_encoded* enc, int32_t batch_index, const int32_t
   });
 }
 
-int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequence, int32_t n_start, const int32_t* text_tokens,
-                    const int32_t* text_offsets, const int32_t* num_frames, int32_t median_filter_width, int32_t* alignments_out,
-                    int32_t capacity_pairs, int32_t* pair_offsets_out, float* text_token_probs_out) {
+int b2w_align_items(b2w_model* h, const b2w_encoded* const* encs, const int32_t* items_in, int32_t n_items,
+                    const int32_t* start_sequence, int32_t n_start, const int32_t* text_tokens, const int32_t* text_offsets,
+                    const int32_t* num_frames, int32_t median_filter_width, int32_t* alignments_out, int32_t capacity_pairs,
+                    int32_t* pair_offsets_out, float* text_token_probs_out) {
   return guarded(h, [&](Model* m) {
-    B2W_CHECK(enc && enc->e && start_sequence && n_start >= 1 && text_offsets && num_frames && pair_offsets_out, "bad arguments");
-    Encoded* e = enc->e;
-    const int B = e->B;
+    B2W_CHECK(encs && items_in && n_items >= 1 && start_sequence && n_start >= 1 && text_offsets && num_frames && pair_offsets_out,
+              "bad arguments");
+    const int B = n_items;
     if (median_filter_width < 1 || median_filter_width % 2 == 0) throw Error("align: median_filter_width must be odd", true);
     if (text_offsets[0] != 0) throw Error("align: text_offsets must start at 0", true);
     for (int b = 0; b < B; ++b)
@@ -2349,6 +2374,11 @@ int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequenc
     int64_t need = 0;
     for (int b = 0; b < B; ++b) {
       AlignItem& it = items[b];
+      B2W_CHECK(encs[b] && encs[b]->e, "align: null encoder output");
+      it.e = encs[b]->e;
+      it.index = items_in[b];
+      if (it.e->owner != m) throw Error("align: the encoder output belongs to another model", true);
+      if (it.index < 0 || it.index >= it.e->B) throw Error("align: batch index out of range", true);
       it.n_text = text_offsets[b + 1] - text_offsets[b];
       it.nf = align_frames(num_frames[b]);
       if (it.n_text == 0) continue;
@@ -2359,7 +2389,7 @@ int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequenc
     }
     if (need > capacity_pairs) throw Error("align: alignment buffer too small: it needs sum(n_text + 1 + nf) pairs", true);
     B2W_CHECK(need == 0 || alignments_out, "bad arguments");
-    if (need > 0) align_run(m, e, 0, start_sequence, n_start, items, median_filter_width);
+    if (need > 0) align_run(m, start_sequence, n_start, items, median_filter_width);
     pair_offsets_out[0] = 0;
     for (int b = 0; b < B; ++b) {
       const std::vector<int2>& p = items[b].pairs;
@@ -2369,6 +2399,60 @@ int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequenc
       }
       pair_offsets_out[b + 1] = pair_offsets_out[b] + (int32_t)p.size();
     }
+  });
+}
+
+int b2w_align_batch(b2w_model* h, b2w_encoded* enc, const int32_t* start_sequence, int32_t n_start, const int32_t* text_tokens,
+                    const int32_t* text_offsets, const int32_t* num_frames, int32_t median_filter_width, int32_t* alignments_out,
+                    int32_t capacity_pairs, int32_t* pair_offsets_out, float* text_token_probs_out) {
+  if (!enc || !enc->e) return guarded([] { B2W_CHECK(false, "bad arguments"); });
+  const std::vector<const b2w_encoded*> encs(enc->e->B, enc);
+  std::vector<int32_t> items(enc->e->B);
+  for (int b = 0; b < enc->e->B; ++b) items[b] = b;
+  return b2w_align_items(h, encs.data(), items.data(), enc->e->B, start_sequence, n_start, text_tokens, text_offsets, num_frames,
+                         median_filter_width, alignments_out, capacity_pairs, pair_offsets_out, text_token_probs_out);
+}
+
+int b2w_encoded_split(b2w_model* h, const b2w_encoded* enc, b2w_encoded** outs) {
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(enc && enc->e && outs, "bad arguments");
+    Encoded* e = enc->e;
+    B2W_CHECK(e->owner == m, "the encoder output belongs to another model");
+    ensure_cross_kv(m, e);
+    const int B = e->B, rows = 2 * m->cfg.n_text_layer;
+    const size_t enc_item = e->enc_bytes / B, seg = e->xkv_bytes / ((size_t)rows * B);  // one (layer, K|V) slice of one item
+    int max_pitch = 0;
+    B2W_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, m->device));
+    std::vector<std::unique_ptr<Encoded>> parts(B);
+    for (int b = 0; b < B; ++b) {
+      Encoded* p = new Encoded;
+      parts[b].reset(p);
+      p->owner = m;
+      p->B = 1;
+      p->enc_bytes = enc_item;
+      p->enc_out = encoded_alloc(m, enc_item);
+      p->xkv_bytes = seg * rows;
+      p->xkv = encoded_alloc(m, p->xkv_bytes);
+      const char* src = reinterpret_cast<const char*>(e->xkv) + b * seg;
+      B2W_CUDA(cudaMemcpyAsync(p->enc_out, reinterpret_cast<const char*>(e->enc_out) + b * enc_item, enc_item,
+                               cudaMemcpyDeviceToDevice, m->stream));
+      if (seg * B <= (size_t)max_pitch) {
+        B2W_CUDA(cudaMemcpy2DAsync(p->xkv, seg, src, seg * B, seg, rows, cudaMemcpyDeviceToDevice, m->stream));
+      } else {
+        for (int r = 0; r < rows; ++r)
+          B2W_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(p->xkv) + r * seg, src + r * seg * B, seg, cudaMemcpyDeviceToDevice,
+                                   m->stream));
+      }
+    }
+    for (int b = 0; b < B; ++b) outs[b] = new b2w_encoded{parts[b].release()};
+  });
+}
+
+int b2w_memory_get(b2w_model* h, int64_t* encoded_bytes, int64_t* pool_bytes) {
+  return guarded(h, [&](Model* m) {
+    B2W_CHECK(encoded_bytes && pool_bytes, "null argument");
+    *encoded_bytes = (int64_t)m->encoded_bytes;
+    *pool_bytes = (int64_t)m->pool_bytes;
   });
 }
 

@@ -64,9 +64,11 @@ struct Model {
   cudaStream_t stream = nullptr;
   std::mutex mu;
   std::vector<void*> allocs;  // allocated once (weights, decoder workspace), freed with the model
-  // size-keyed free list for encoder outputs / cross-KV caches: a 3.9 GB cudaMalloc+cudaFree per call costs ~100s of ms
+  // size-keyed free list for encoder outputs / cross-KV caches: a 3.9 GB cudaMalloc+cudaFree per call costs ~100s of ms, and a
+  // cudaFree synchronises the device
   std::vector<std::pair<size_t, void*>> pool;
   size_t pool_bytes = 0;
+  size_t encoded_bytes = 0;  // device bytes of the live encoder outputs (b2w_memory_get)
   void* pool_get(size_t bytes);
   void pool_put(void* p, size_t bytes);
 

@@ -143,8 +143,8 @@ GV_QKV, GV_F16, GV_GELU_F16, GV_RESID_LN, GV_F32 = range(5)
 ABI_SYMBOLS = (
     "b2w_last_error", "b2w_abi_version", "b2w_device_count", "b2w_model_create", "b2w_model_destroy",
     "b2w_model_info", "b2w_model_sync", "b2w_logmel", "b2w_logmel_frames", "b2w_encode", "b2w_encode_audio",
-    "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_generate", "b2w_gen_opts_default",
-    "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
+    "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_encoded_split", "b2w_memory_get", "b2w_generate",
+    "b2w_gen_opts_default", "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_align_items", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
     "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
     "b2w_debug_step_logits", "b2w_debug_self_attn", "b2w_debug_cross_attn", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
     "b2w_session_create", "b2w_session_push", "b2w_session_run", "b2w_session_pending", "b2w_session_counters", "b2w_session_destroy",
@@ -187,6 +187,8 @@ def load_library():
         lib.b2w_encoded_to_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b2w_encoded_free.argtypes = [C.c_void_p]
         lib.b2w_encoded_free.restype = None
+        lib.b2w_encoded_split.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
+        lib.b2w_memory_get.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         lib.b2w_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(_GenOpts),
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b2w_gen_opts_default.argtypes = [C.POINTER(_GenOpts)]
@@ -196,6 +198,8 @@ def load_library():
                                   C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]
         lib.b2w_align_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                         C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        lib.b2w_align_items.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         lib.b2w_model_set_alignment_heads.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         lib.b2w_timing_enable.argtypes = [C.c_void_p, C.c_int32]
         lib.b2w_timing_reset.argtypes = [C.c_void_p]
@@ -480,6 +484,9 @@ class Whisper:
             self._rr += 1
             return r
 
+    def _pick_replica(self, replica: Optional[int]) -> _Replica:
+        return self._next_replica() if replica is None else self._replicas[replica]
+
     def _replica_for(self, sv: StorageView) -> _Replica:
         return getattr(sv, "_replica", None) or self._replicas[0]
 
@@ -504,14 +511,15 @@ class Whisper:
         self._replicas, fresh._replicas = fresh._replicas, []
 
     # ---- encode (transcribe.py:209,1400) ----
-    def encode(self, features: Union[StorageView, np.ndarray], to_cpu: bool = False) -> StorageView:
+    def encode(self, features: Union[StorageView, np.ndarray], to_cpu: bool = False, replica: Optional[int] = None) -> StorageView:
+        """``replica``: the replica (index) that encodes and holds the output; None takes the next one in round-robin order."""
         arr = features.numpy() if isinstance(features, StorageView) else np.asarray(features)
         if arr.dtype != np.float32 or not arr.flags["C_CONTIGUOUS"]:
             arr = np.ascontiguousarray(arr, dtype=np.float32)
         if arr.ndim != 3 or arr.shape[1] != self.dims.n_mels or arr.shape[2] != 3000:
             raise ValueError(f"Invalid input features shape: expected an input with shape (batch, {self.dims.n_mels}, 3000), "
                              f"but got an input with shape {tuple(arr.shape)} instead")
-        rep = self._next_replica()
+        rep = self._pick_replica(replica)
         h = C.c_void_p()
         with rep.lock:
             _check(rep._lib.b2w_encode(rep.handle, _ptr(arr), arr.shape[0], C.byref(h)))
@@ -522,11 +530,11 @@ class Whisper:
             return StorageView.from_array(sv.numpy())
         return sv
 
-    def encode_audio(self, chunks: Sequence[np.ndarray], return_features: bool = False):
+    def encode_audio(self, chunks: Sequence[np.ndarray], return_features: bool = False, replica: Optional[int] = None):
         """Fused log-mel + encoder for <=30 s chunks (the batched pipeline's hot path): PCM in, encoder output
         resident on the device.  Mirrors ``feature_extractor(chunk)[..., :-1]`` + ``pad_or_trim`` + ``encode``
-        (transcribe.py:463-467,514-516,209)."""
-        rep = self._next_replica()
+        (transcribe.py:463-467,514-516,209).  ``replica`` as in ``encode``."""
+        rep = self._pick_replica(replica)
         arrs = [np.ascontiguousarray(c, dtype=np.float32) for c in chunks]
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data if a.size else None for a in arrs])
@@ -599,11 +607,13 @@ class Whisper:
                      repetition_penalty: float = 1, no_repeat_ngram_size: int = 0, max_length: int = 448, return_scores: bool = False,
                      return_no_speech_prob: bool = False, max_initial_timestamp_index: int = 50, suppress_blank: bool = True,
                      suppress_tokens: Optional[Sequence[int]] = (-1,), sampling_topk: int = 1, sampling_temperature: float = 1,
-                     seed: int = 0, slots: int = 0, replica: int = 0) -> "DecodeQueue":
+                     seed: int = 0, slots: int = 0, replica: Optional[int] = 0) -> "DecodeQueue":
         """A continuous-batching decoder with ``generate``'s options: ``push`` items, iterate ``(item_id, WhisperGenerationResult)``
         in completion order.  A finished item's rows take the next queued item instead of idling until a whole batch ends.
-        ``slots``: chunks decoded at once (0: as many as one decode step takes, 80 // rows per chunk)."""
-        rep = self._replicas[replica]
+        ``slots``: chunks decoded at once (0: as many as one decode step takes, 80 // rows per chunk).  ``replica``: the replica
+        (index) that decodes, and whose encoder outputs ``push`` takes (the queue's ``replica``); None takes the next one in
+        round-robin order."""
+        rep = self._pick_replica(replica)
         o, sup_arr = _gen_opts(rep._lib, self.dims.n_text_ctx, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
                                length_penalty=length_penalty, repetition_penalty=repetition_penalty,
                                no_repeat_ngram_size=no_repeat_ngram_size, max_length=max_length, return_scores=return_scores,
@@ -631,29 +641,77 @@ class Whisper:
             out.append([(f"<|{names[i]}|>", float(probs[b, i])) for i in order])
         return out
 
+    def split_encoded(self, storage_view: StorageView) -> List[StorageView]:
+        """One single-item device encoder output per batch item of ``storage_view`` (from ``encode`` or ``encode_audio``), each a
+        bit-identical copy in device memory of its own: a chunk's output can then be freed as soon as that chunk is done, whatever
+        the rest of its batch does.  ``storage_view`` is unchanged."""
+        if not isinstance(storage_view, StorageView) or storage_view._handle is None:
+            raise ValueError("split_encoded takes a device encoder output (a StorageView from encode / encode_audio)")
+        rep = self._replica_for(storage_view)
+        B = storage_view.shape[0]
+        hs = (C.c_void_p * B)()
+        with rep.lock:
+            _check(rep._lib.b2w_encoded_split(rep.handle, storage_view._handle, hs))
+        out = []
+        for b in range(B):
+            sv = StorageView(handle=C.c_void_p(hs[b]), owner=self, shape=(1, self.dims.n_audio_ctx, self.dims.n_audio_state))
+            sv._replica = rep
+            rep.track_output(sv)
+            out.append(sv)
+        return out
+
+    def memory(self, replica: int = 0) -> Dict[str, int]:
+        """Device bytes of this model's live encoder outputs (``encoded_bytes``, including those only a decode queue still holds)
+        and of the buffers parked in its pool for reuse (``pool_bytes``)."""
+        rep = self._replicas[replica]
+        enc, pool = C.c_int64(), C.c_int64()
+        with rep.lock:
+            _check(rep._lib.b2w_memory_get(rep.handle, C.byref(enc), C.byref(pool)))
+        return dict(encoded_bytes=int(enc.value), pool_bytes=int(pool.value))
+
     # ---- align (transcribe.py:1709-1715) ----
     def align(self, features, start_sequence, text_tokens, num_frames, *, median_filter_width: int = 7):
         """``ctranslate2.models.Whisper.align`` (transcribe.py:1709-1715): one result per batch item with ``.alignments``
         (list of (text_token_index, time_index)) and ``.text_token_probs``."""
         enc = self._as_encoded(features)
-        rep = self._replica_for(enc)
-        start = np.ascontiguousarray(list(start_sequence), dtype=np.int32)
         if len(text_tokens) != enc.shape[0]:
             raise ValueError("align: one text token list per batch item is required")
         B = enc.shape[0]
+        frames = [num_frames[b] if isinstance(num_frames, (list, tuple)) else num_frames for b in range(B)]
+        return self.align_items([(enc, b) for b in range(B)], start_sequence, text_tokens, frames, median_filter_width=median_filter_width)
+
+    def align_items(self, pairs: Sequence[Tuple[StorageView, int]], start_sequence, text_tokens, num_frames, *,
+                    median_filter_width: int = 7) -> List[WhisperAlignmentResult]:
+        """``align`` over items of several encoder outputs: item j is batch index ``pairs[j][1]`` of the device encoder output
+        ``pairs[j][0]``, with ``text_tokens[j]`` and ``num_frames[j]``.  One result per item, in order."""
+        pairs = list(pairs)
+        B = len(pairs)
+        if len(text_tokens) != B or len(num_frames) != B:
+            raise ValueError("align_items: one text token list and one frame count per item are required")
+        if B == 0:
+            return []
+        for sv, _ in pairs:
+            if not isinstance(sv, StorageView) or sv._handle is None:
+                raise ValueError("align_items takes device encoder outputs (StorageViews from encode / encode_audio)")
+        rep = self._replica_for(pairs[0][0])
+        if any(self._replica_for(sv) is not rep for sv, _ in pairs):
+            raise ValueError("align_items: every encoder output must belong to one replica")
+        encs = (C.c_void_p * B)(*[sv._handle.value for sv, _ in pairs])
+        items = np.ascontiguousarray([int(i) for _, i in pairs], np.int32)
+        start = np.ascontiguousarray(list(start_sequence), dtype=np.int32)
         texts = [np.asarray(list(t), dtype=np.int32) for t in text_tokens]
-        frames = np.ascontiguousarray([int(num_frames[b] if isinstance(num_frames, (list, tuple)) else num_frames) for b in range(B)], np.int32)
+        frames = np.ascontiguousarray([int(f) for f in num_frames], np.int32)
         offsets = np.zeros(B + 1, np.int32)
         offsets[1:] = np.cumsum([len(t) for t in texts])
         toks = np.ascontiguousarray(np.concatenate(texts) if offsets[-1] else np.zeros(1, np.int32), dtype=np.int32)
         cap = int(sum(len(t) + max(1, min(1500, nf // 2)) + 1 for t, nf in zip(texts, frames) if len(t)))
-        pairs = np.zeros((max(1, cap), 2), np.int32)
+        out_pairs = np.zeros((max(1, cap), 2), np.int32)
         pair_offsets = np.zeros(B + 1, np.int32)
         probs = np.zeros(max(1, int(offsets[-1])), np.float32)
         with rep.lock:
-            _check(rep._lib.b2w_align_batch(rep.handle, enc._handle, _ptr(start), len(start), _ptr(toks), _ptr(offsets), _ptr(frames),
-                                            int(median_filter_width), _ptr(pairs), cap, _ptr(pair_offsets), _ptr(probs)))
-        return [WhisperAlignmentResult([tuple(p) for p in pairs[pair_offsets[b]:pair_offsets[b + 1]].tolist()],
+            _check(rep._lib.b2w_align_items(rep.handle, encs, _ptr(items), B, _ptr(start), len(start), _ptr(toks), _ptr(offsets),
+                                            _ptr(frames), int(median_filter_width), _ptr(out_pairs), cap, _ptr(pair_offsets), _ptr(probs)))
+        return [WhisperAlignmentResult([tuple(p) for p in out_pairs[pair_offsets[b]:pair_offsets[b + 1]].tolist()],
                                        probs[offsets[b]:offsets[b + 1]].tolist()) for b in range(B)]
 
     def set_alignment_heads(self, heads=None):
@@ -766,6 +824,7 @@ class DecodeQueue:
 
     def __init__(self, owner: "Whisper", rep: _Replica, opts: _GenOpts, sup_arr: np.ndarray, slots: int = 0):
         self._owner, self._rep, self._opts, self._sup = owner, rep, opts, sup_arr
+        self.replica = owner._replicas.index(rep)
         self._return_scores = bool(opts.return_scores)
         self._return_ns = bool(opts.return_no_speech_prob)
         h, slots = C.c_void_p(), C.c_int32(int(slots))

@@ -244,8 +244,14 @@ class _LanguageVote:
 # batched pipeline (transcribe.py:111-617)
 # --------------------------------------------------------------------------------------------------
 class BatchedInferencePipeline:
-    def __init__(self, model):
+    def __init__(self, model, continuous_batching: bool = False):
+        """`continuous_batching`: decode `transcribe` / `transcribe_many` through one decode queue per call (``Whisper.decode_queue``)
+        instead of one ``generate`` call per batch, so a finished chunk's rows take the next chunk instead of idling until the
+        batch's longest chunk ends.  Segments come out in the same order; because the queue groups the chunks differently, near-ties
+        of the search may resolve differently than with one ``generate`` per batch.  With several engine replicas (a `device_index`
+        list, or `num_workers` > 1) each call decodes on one replica, the next in round-robin order, and encodes all its chunks there."""
         self.model: WhisperModel = model
+        self.continuous_batching = continuous_batching
         self.last_speech_timestamp = 0.0
 
     # -- one batch: encode + one generate call + timestamp splitting ---------------------------------
@@ -258,19 +264,9 @@ class BatchedInferencePipeline:
         model = self.model
         batch_results, frame_counts = [], []
         for meta, out, tok in zip(chunks_metadata, outputs, tokenizers):
-            n_frames = int(ceil(meta["duration"]) * model.frames_per_second)
-            frame_counts.append(n_frames)
-            pieces, _, _ = model._split_segments_by_timestamps(
-                tokenizer=tok, tokens=out["tokens"], time_offset=meta["offset"], segment_size=n_frames,
-                segment_duration=meta["duration"], seek=0)
-            rows = []
-            for piece in pieces:
-                text = tok.decode(piece["tokens"])
-                rows.append(dict(
-                    text=text, avg_logprob=out["avg_logprob"], no_speech_prob=out["no_speech_prob"], tokens=piece["tokens"],
-                    start=piece["start"], end=piece["end"], compression_ratio=get_compression_ratio(text),
-                    seek=int(meta["offset"] * model.frames_per_second)))
+            rows, n_frames = self._chunk_rows(meta, out, tok)
             batch_results.append(rows)
+            frame_counts.append(n_frames)
         if options.word_timestamps:
             ends = last_speech if last_speech is not None else {0: self.last_speech_timestamp}
             # one align call per distinct start sequence (it holds the language token), items of other languages empty
@@ -282,16 +278,65 @@ class BatchedInferencePipeline:
                 for i, r in enumerate(model.model.align(encoder_output, list(start), text_tokens, frame_counts, median_filter_width=7)):
                     if mine[i]:
                         aligned[i] = r
-            # words per recording, in chunk order, each with its own tokenizer and running end of speech
-            files = [meta.get("file", 0) for meta in chunks_metadata]
-            for f in dict.fromkeys(files):
-                idx = [i for i, g in enumerate(files) if g == f]
-                ends[f] = model.assemble_words(
-                    [batch_results[i] for i in idx], tokenizers[idx[0]], [aligned[i] for i in idx], options.prepend_punctuations,
-                    options.append_punctuations, ends.get(f, 0.0))
+            self._assemble_words(batch_results, tokenizers, aligned, chunks_metadata, options, ends)
             if last_speech is None:
                 self.last_speech_timestamp = ends[0]
         return batch_results
+
+    def _chunk_rows(self, meta, out, tok):
+        """One decoded chunk's rows (its pieces between timestamp pairs), and its frame count for the alignment."""
+        model = self.model
+        n_frames = int(ceil(meta["duration"]) * model.frames_per_second)
+        pieces, _, _ = model._split_segments_by_timestamps(
+            tokenizer=tok, tokens=out["tokens"], time_offset=meta["offset"], segment_size=n_frames,
+            segment_duration=meta["duration"], seek=0)
+        rows = []
+        for piece in pieces:
+            text = tok.decode(piece["tokens"])
+            rows.append(dict(
+                text=text, avg_logprob=out["avg_logprob"], no_speech_prob=out["no_speech_prob"], tokens=piece["tokens"],
+                start=piece["start"], end=piece["end"], compression_ratio=get_compression_ratio(text),
+                seek=int(meta["offset"] * model.frames_per_second)))
+        return rows, n_frames
+
+    def _assemble_words(self, results, tokenizers, aligned, chunks_metadata, options, ends: dict) -> None:
+        """Words of consecutive chunks from their alignments, per recording in chunk order, each with its own tokenizer and the
+        running end of speech `ends[recording]`, updated in place."""
+        files = [meta.get("file", 0) for meta in chunks_metadata]
+        for f in dict.fromkeys(files):
+            idx = [i for i, g in enumerate(files) if g == f]
+            ends[f] = self.model.assemble_words(
+                [results[i] for i in idx], tokenizers[idx[0]], [aligned[i] for i in idx], options.prepend_punctuations,
+                options.append_punctuations, ends.get(f, 0.0))
+
+    def _prompts(self, tokenizers, options: TranscriptionOptions) -> List[List[int]]:
+        """One decoder prompt per chunk (each its own list)."""
+        made = {}
+        for tok in tokenizers:
+            if id(tok) not in made:
+                history = tok.encode(options.initial_prompt) if options.initial_prompt is not None else []
+                made[id(tok)] = self.model.get_prompt(tok, previous_tokens=history, without_timestamps=options.without_timestamps,
+                                                      hotwords=options.hotwords)
+        return [list(made[id(tok)]) for tok in tokenizers]
+
+    def _detected_languages_into(self, encoder_output, prompts, tokenizers) -> None:
+        """multilingual=True: each prompt's language token becomes the language detected on its chunk."""
+        for row, tok, langs in zip(prompts, tokenizers, self.model.model.detect_language(encoder_output)):
+            row[row.index(tok.language)] = tok.tokenizer.token_to_id(langs[0][0])
+
+    @staticmethod
+    def _output(r, options: TranscriptionOptions) -> dict:
+        toks = r.sequences_ids[0]
+        return dict(avg_logprob=_score_to_avg_logprob(r.scores[0], len(toks), options.length_penalty),
+                    no_speech_prob=r.no_speech_prob, tokens=toks)
+
+    @staticmethod
+    def _search_options(options: TranscriptionOptions) -> dict:
+        """The search options of every decode, as `generate` and a decode queue take them."""
+        return dict(beam_size=options.beam_size, patience=options.patience, length_penalty=options.length_penalty,
+                    suppress_blank=options.suppress_blank, suppress_tokens=options.suppress_tokens, return_scores=True,
+                    return_no_speech_prob=True, sampling_temperature=options.temperatures[0],
+                    repetition_penalty=options.repetition_penalty, no_repeat_ngram_size=options.no_repeat_ngram_size)
 
     def generate_segment_batched(self, features, tokenizer, options: TranscriptionOptions):
         """`features` is either the stacked float32 array [n, n_mels, 3000] (reference contract) or an encoder
@@ -300,30 +345,13 @@ class BatchedInferencePipeline:
         model = self.model
         n = features.shape[0]
         tokenizers = list(tokenizer) if isinstance(tokenizer, (list, tuple)) else [tokenizer] * n
-        made = {}
-        for tok in tokenizers:
-            if id(tok) not in made:
-                history = tok.encode(options.initial_prompt) if options.initial_prompt is not None else []
-                made[id(tok)] = model.get_prompt(tok, previous_tokens=history, without_timestamps=options.without_timestamps,
-                                                 hotwords=options.hotwords)
-        prompts = [list(made[id(tok)]) for tok in tokenizers]
+        prompts = self._prompts(tokenizers, options)
         max_length = _check_max_length(len(prompts[0]), options.max_new_tokens, model.max_length)
         encoder_output = features if isinstance(features, engine.StorageView) else model.encode(features)
         if options.multilingual:
-            for row, tok, langs in zip(prompts, tokenizers, model.model.detect_language(encoder_output)):
-                row[row.index(tok.language)] = tok.tokenizer.token_to_id(langs[0][0])
-        results = model.model.generate(
-            encoder_output, prompts, beam_size=options.beam_size, patience=options.patience,
-            length_penalty=options.length_penalty, max_length=max_length, suppress_blank=options.suppress_blank,
-            suppress_tokens=options.suppress_tokens, return_scores=True, return_no_speech_prob=True,
-            sampling_temperature=options.temperatures[0], repetition_penalty=options.repetition_penalty,
-            no_repeat_ngram_size=options.no_repeat_ngram_size)
-        outputs = []
-        for r in results:
-            toks = r.sequences_ids[0]
-            outputs.append(dict(avg_logprob=_score_to_avg_logprob(r.scores[0], len(toks), options.length_penalty),
-                                no_speech_prob=r.no_speech_prob, tokens=toks))
-        return encoder_output, outputs
+            self._detected_languages_into(encoder_output, prompts, tokenizers)
+        results = model.model.generate(encoder_output, prompts, max_length=max_length, **self._search_options(options))
+        return encoder_output, [self._output(r, options) for r in results]
 
     def transcribe(
         self,
@@ -370,11 +398,20 @@ class BatchedInferencePipeline:
         reference (transcribe.py:254-375).  Returns (lazy segment generator, TranscriptionInfo)."""
         kw = {k: v for k, v in locals().items() if k not in ("self", "audio", "clip_timestamps")}
         plan = self._prepare([audio], [clip_timestamps], kw)[0]
-        segments = (seg for _, seg in self._batched_segments_generator(
-            plan.chunks, [plan.tokenizer] * len(plan.chunks), plan.metadata, batch_size, plan.options, log_progress))
+        return self._lazy_segments(plan, batch_size, log_progress), plan.info
+
+    def _lazy_segments(self, plan: _FilePlan, batch_size, log_progress) -> Iterator[Segment]:
+        """`transcribe`'s segment generator.  Closing it closes the decoding generator at once (a decode queue's session holds
+        device memory), rather than when the garbage collector gets to it."""
+        pairs = self._segments_generator(plan.chunks, [plan.tokenizer] * len(plan.chunks), plan.metadata, batch_size, plan.options,
+                                         log_progress)
+        segments = (seg for _, seg in pairs)
         if not plan.from_user:
             segments = restore_speech_timestamps(segments, plan.spans, self.model.feature_extractor.sampling_rate)
-        return segments, plan.info
+        try:
+            yield from segments
+        finally:
+            pairs.close()
 
     def transcribe_many(self, audios: Sequence[Union[str, BinaryIO, np.ndarray]],
                         clip_timestamps: Optional[Sequence[Optional[List[dict]]]] = None,
@@ -408,8 +445,8 @@ class BatchedInferencePipeline:
             metadata += [dict(m, file=fi) for m in p.metadata]
             tokenizers += [p.tokenizer] * len(p.chunks)
         segments = [[] for _ in plans]
-        for fi, seg in self._batched_segments_generator(chunks, tokenizers, metadata, kw["batch_size"], plans[0].options,
-                                                        kw["log_progress"], last_speech={}):
+        for fi, seg in self._segments_generator(chunks, tokenizers, metadata, kw["batch_size"], plans[0].options, kw["log_progress"],
+                                                last_speech={}):
             segments[fi].append(seg)
         sr = self.model.feature_extractor.sampling_rate
         return [(segs if p.from_user else list(restore_speech_timestamps(segs, p.spans, sr)), p.info)
@@ -535,6 +572,37 @@ class BatchedInferencePipeline:
         chunks, metadata = collect_chunks(audio, spans, max_duration=chunk_length)
         return _FilePlan(chunks, metadata, spans, from_user=False)
 
+    def _segments_generator(self, features, tokenizers, chunks_metadata, batch_size, options, log_progress,
+                            last_speech: Optional[dict] = None):
+        gen = self._continuous_segments_generator if self.continuous_batching else self._batched_segments_generator
+        return gen(features, tokenizers, chunks_metadata, batch_size, options, log_progress, last_speech)
+
+    def _encode_block(self, block, replica: Optional[int] = None):
+        """Encoder output of a list of PCM chunks: the fused audio path, or features first when a chunk is longer than 30 s.
+        `replica`: the engine replica that must hold the output (a decode queue's); None leaves the choice to the engine."""
+        pin = {} if replica is None else dict(replica=replica)
+        if any(len(c) > 30 * self.model.feature_extractor.sampling_rate for c in block):
+            # the reference's order of operations (transcribe.py:463-467,514-516): log-mel of the whole clip — its clamp maximum and
+            # its last frames see the audio beyond 30 s — then pad_or_trim of the features
+            fe = self.model.feature_extractor
+            feats = np.stack([pad_or_trim(fe(c)[..., :-1]) for c in block])
+            if not pin:
+                return self.model.encode(feats)
+            return self.model.model.encode(get_ctranslate2_storage(feats), to_cpu=False, **pin)
+        return self.model.model.encode_audio(block, **pin)
+
+    @staticmethod
+    def _chunk_segments(rows, meta, options, seg_ids: dict):
+        """(recording index, Segment) of one chunk's rows; segment ids count per recording in `seg_ids`."""
+        f = meta.get("file", 0)
+        for row in rows:
+            seg_ids[f] = seg_ids.get(f, 0) + 1
+            yield f, Segment(
+                seek=row["seek"], id=seg_ids[f], text=row["text"], start=round(row["start"], 3), end=round(row["end"], 3),
+                words=[Word(**w) for w in row["words"]] if options.word_timestamps else None, tokens=row["tokens"],
+                avg_logprob=row["avg_logprob"], no_speech_prob=row["no_speech_prob"],
+                compression_ratio=row["compression_ratio"], temperature=options.temperatures[0])
+
     def _batched_segments_generator(self, features, tokenizers, chunks_metadata, batch_size, options, log_progress,
                                     last_speech: Optional[dict] = None):
         """`features`: list of PCM chunks (fused audio->mel->encoder path, the default here) or the reference's
@@ -549,26 +617,94 @@ class BatchedInferencePipeline:
         for lo in range(0, total, batch_size):
             block = features[lo : lo + batch_size]
             if fused:
-                if any(len(c) > 30 * self.model.feature_extractor.sampling_rate for c in block):
-                    # the reference's order of operations (transcribe.py:463-467,514-516): log-mel of the whole clip — its clamp maximum and
-                    # its last frames see the audio beyond 30 s — then pad_or_trim of the features
-                    fe = self.model.feature_extractor
-                    block = self.model.encode(np.stack([pad_or_trim(fe(c)[..., :-1]) for c in block]))
-                else:
-                    block = self.model.model.encode_audio(block)
+                block = self._encode_block(block)
             metas = chunks_metadata[lo : lo + batch_size]
             for meta, rows in zip(metas, self.forward(block, tokenizers[lo : lo + batch_size], metas, options, last_speech)):
-                f = meta.get("file", 0)
-                for row in rows:
-                    seg_ids[f] = seg_ids.get(f, 0) + 1
-                    yield f, Segment(
-                        seek=row["seek"], id=seg_ids[f], text=row["text"], start=round(row["start"], 3), end=round(row["end"], 3),
-                        words=[Word(**w) for w in row["words"]] if options.word_timestamps else None, tokens=row["tokens"],
-                        avg_logprob=row["avg_logprob"], no_speech_prob=row["no_speech_prob"],
-                        compression_ratio=row["compression_ratio"], temperature=options.temperatures[0])
+                yield from self._chunk_segments(rows, meta, options, seg_ids)
                 bar.update(1)
         bar.close()
         self.last_speech_timestamp = 0.0
+
+    def _continuous_segments_generator(self, chunks, tokenizers, chunks_metadata, batch_size, options, log_progress,
+                                       last_speech: Optional[dict] = None):
+        """`_batched_segments_generator` through one decode queue (PCM chunks only).  The queue decodes `slots` chunks at once
+        (at most `batch_size`, and as many as one decode step takes).  Chunks are encoded `slots` at a time, each batch split into
+        per-chunk encoder outputs so a chunk's device memory goes as soon as it is done, and a batch is encoded only while fewer than
+        `slots` chunks wait beyond those the slots hold (a finished chunk's slot holds it until the next `run` rebinds the slot):
+        fewer than 3 x slots chunk encodings are then alive at any time, however unequal the chunks' lengths.  Finished chunks are
+        aligned (word timestamps) after each `run`, then wait on the host until every earlier chunk has been emitted."""
+        from tqdm import tqdm
+
+        model = self.model
+        total = len(chunks)
+        bar = tqdm(total=total, disable=not log_progress, position=0)
+        seg_ids = {}
+        ends = last_speech if last_speech is not None else {0: self.last_speech_timestamp}
+        queue = None
+        try:
+            if total == 0:
+                return
+            prompts = self._prompts(tokenizers, options)
+            max_lengths = [_check_max_length(len(p), options.max_new_tokens, model.max_length) for p in prompts]
+            # the queue decodes on one replica (the next in round-robin order), so every batch is encoded on that replica too
+            queue = model.model.decode_queue(max_length=model.max_length, slots=batch_size, replica=None,
+                                             **self._search_options(options))
+            slots = queue.slots
+            chunk_of = {}       # queue item id -> chunk index
+            encodings = {}      # chunk index -> its encoder output, kept for the alignment (word timestamps)
+            finished = {}       # chunk index -> (rows, alignment) of a decoded chunk not yet emitted
+            encoded = emitted = held = 0
+            while emitted < total:
+                while encoded < total and queue.pending() + held - slots < slots:
+                    lo, hi = encoded, min(total, encoded + slots)
+                    batch = self._encode_block(chunks[lo:hi], replica=queue.replica)
+                    if options.multilingual:
+                        self._detected_languages_into(batch, prompts[lo:hi], tokenizers[lo:hi])
+                    parts = model.model.split_encoded(batch)
+                    del batch
+                    for c, part in zip(range(lo, hi), parts):
+                        (item,) = queue.push(part, [prompts[c]], [max_lengths[c]])
+                        chunk_of[item] = c
+                        if options.word_timestamps:
+                            encodings[c] = part
+                    del parts, part  # the queue (and `encodings`) hold what is still needed
+                    encoded = hi
+                done = queue.run()
+                if not done:
+                    raise RuntimeError("the decode queue ran dry before every chunk was decoded")
+                held = len(done)
+                new = []
+                for item, r in done:
+                    c = chunk_of.pop(item)
+                    rows, n_frames = self._chunk_rows(chunks_metadata[c], self._output(r, options), tokenizers[c])
+                    finished[c] = [rows, None, n_frames]
+                    new.append(c)
+                if options.word_timestamps and new:
+                    for start in dict.fromkeys(tuple(tokenizers[c].sot_sequence) for c in new):
+                        mine = [c for c in new if tuple(tokenizers[c].sot_sequence) == start]
+                        aligned = model.model.align_items(
+                            [(encodings[c], 0) for c in mine], list(start),
+                            [model.text_tokens(finished[c][0], tokenizers[c].eot) for c in mine], [finished[c][2] for c in mine],
+                            median_filter_width=7)
+                        for c, a in zip(mine, aligned):
+                            finished[c][1] = a
+                    for c in new:
+                        del encodings[c]
+                while emitted in finished:
+                    rows, aligned, _ = finished.pop(emitted)
+                    meta = chunks_metadata[emitted]
+                    if options.word_timestamps:
+                        self._assemble_words([rows], [tokenizers[emitted]], [aligned], [meta], options, ends)
+                        if last_speech is None:
+                            self.last_speech_timestamp = ends[0]
+                    yield from self._chunk_segments(rows, meta, options, seg_ids)
+                    bar.update(1)
+                    emitted += 1
+        finally:
+            if queue is not None:
+                queue.close()
+            bar.close()
+            self.last_speech_timestamp = 0.0
 
 
 # --------------------------------------------------------------------------------------------------

@@ -109,6 +109,13 @@ int b2w_encoded_shape(const b2w_encoded* e, int64_t shape_out[3]);
 /* to_cpu=True / debugging: copy [batch, 1500, d] out as float32. */
 int b2w_encoded_to_host(b2w_model* m, const b2w_encoded* e, float* out);
 void b2w_encoded_free(b2w_encoded* e);
+/* One single-item encoder output per batch item of e: outs[b] receives item b, bit for bit (encoder output [1, 1500, d] and
+ * cross-attention K/V [L][K|V][1][H][1500][64]), in device memory of its own, so each can be freed on its own.  e is not
+ * changed (its cross-attention K/V is computed first when no decode has yet), and the caller still frees it. */
+int b2w_encoded_split(b2w_model* m, const b2w_encoded* e, b2w_encoded** outs);
+/* Device bytes of the model's live encoder outputs (including those only a decode session still holds) and bytes parked in
+ * its buffer pool for reuse. */
+int b2w_memory_get(b2w_model* m, int64_t* encoded_bytes, int64_t* pool_bytes);
 
 /* ---- decoder ------------------------------------------------------------------------------------
  * Whisper.generate(encoder_output, prompts, **opts) -> [WhisperGenerationResult] (transcribe.py:222-236,
@@ -179,6 +186,13 @@ int b2w_align(b2w_model* m, b2w_encoded* e, int32_t batch_index, const int32_t* 
 int b2w_align_batch(b2w_model* m, b2w_encoded* e, const int32_t* start_sequence, int32_t n_start,
                     const int32_t* text_tokens, const int32_t* text_offsets, const int32_t* num_frames,
                     int32_t median_filter_width, int32_t* alignments_out, int32_t capacity_pairs,
+                    int32_t* pair_offsets_out, float* text_token_probs_out);
+/* b2w_align_batch over items of several encoder outputs: item j is batch index items[j] of encs[j], and
+ * text_offsets / num_frames / pair_offsets_out / probabilities are indexed by j as b2w_align_batch indexes them by b.
+ * b2w_align_batch is this call with encs[j] = e and items[j] = j. */
+int b2w_align_items(b2w_model* m, const b2w_encoded* const* encs, const int32_t* items, int32_t n_items,
+                    const int32_t* start_sequence, int32_t n_start, const int32_t* text_tokens, const int32_t* text_offsets,
+                    const int32_t* num_frames, int32_t median_filter_width, int32_t* alignments_out, int32_t capacity_pairs,
                     int32_t* pair_offsets_out, float* text_token_probs_out);
 
 /* config.json "alignment_heads" of a converted model (transcribe.py:700-710 reads the model directory): n_pairs
