@@ -114,5 +114,7 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 // ---- TMA descriptor creation (driver entry point fetched at run time: no link-time libcuda) ----------
 CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box);
+// the same for 8-bit elements (e4m3 codes): a 128-byte swizzle row holds 128 of them
+CUtensorMap make_tmap_u8(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box);
 
 }  // namespace b2w

@@ -101,8 +101,8 @@ Model::~Model() {
   for (void* p : allocs) cudaFree(p);
   for (auto& it : pool) cudaFree(it.second);
   // the buffers that are reallocated when a larger shape arrives
-  void* ws[] = {e_feats, e_x0, e_x1, e_x, e_xn, e_qkv, e_ao, e_h, e_pcm, e_chunks, e_chunk_max, kcache, vcache, d_xpart, sb_blob,
-                d_align_heads};
+  void* ws[] = {e_feats, e_x0, e_x1, e_x, e_xn, e_qkv, e_ao, e_h, e_q, e_qs, e_pcm, e_chunks, e_chunk_max, kcache, vcache, d_xpart,
+                sb_blob, d_align_heads};
   for (void* p : ws)
     if (p) cudaFree(p);
   if (h_pinned) cudaFreeHost(h_pinned);
@@ -399,6 +399,24 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
     L.w2 = up.f16(tt, p + ".mlp.2.weight", {d, 4 * d});
     L.b2 = up.f32(tt, p + ".mlp.2.bias", {d});
   }
+  if (m->fp8_enc) {
+    // e4m3 codes + per-channel scales from the fp16 values the float16 path multiplies with; the fp16 copies are released
+    auto to_e4m3 = [&](__half*& w, int N, int K, uint8_t*& q, float*& sc) {
+      q = up.alloc<uint8_t>((size_t)N * K);
+      sc = up.alloc<float>((size_t)N);
+      quantize_rows_e4m3(w, q, sc, N, K, m->stream);
+      B2W_CUDA(cudaStreamSynchronize(m->stream));
+      m->allocs.erase(std::find(m->allocs.begin(), m->allocs.end(), (void*)w));
+      B2W_CUDA(cudaFree(w));
+      w = nullptr;
+    };
+    for (EncLayerW& L : m->enc) {
+      to_e4m3(L.wqkv, 3 * d, d, L.q_wqkv, L.s_wqkv);
+      to_e4m3(L.wo, d, d, L.q_wo, L.s_wo);
+      to_e4m3(L.w1, 4 * d, d, L.q_w1, L.s_w1);
+      to_e4m3(L.w2, d, 4 * d, L.q_w2, L.s_w2);
+    }
+  }
   m->enc_lnp_g = up.f32(tt, "encoder.ln_post.weight", {d});
   m->enc_lnp_b = up.f32(tt, "encoder.ln_post.bias", {d});
 
@@ -601,7 +619,7 @@ static void build_model(Model* m, const b2w_config& cfg, const TensorTable& tt) 
 static void ensure_encoder_ws(Model* m, int b) {
   if (b <= m->enc_max_b) return;
   B2W_CUDA(cudaStreamSynchronize(m->stream));
-  void* old[] = {m->e_feats, m->e_x0, m->e_x1, m->e_x, m->e_xn, m->e_qkv, m->e_ao, m->e_h, m->e_chunks, m->e_chunk_max};
+  void* old[] = {m->e_feats, m->e_x0, m->e_x1, m->e_x, m->e_xn, m->e_qkv, m->e_ao, m->e_h, m->e_q, m->e_qs, m->e_chunks, m->e_chunk_max};
   for (void* p : old)
     if (p) cudaFree(p);
   m->enc_plans.clear();
@@ -614,6 +632,8 @@ static void ensure_encoder_ws(Model* m, int b) {
   m->e_qkv = dalloc<__half>(M * 3 * d);
   m->e_ao = dalloc<__half>(M * d);
   m->e_h = dalloc<__half>(M * 4 * d);
+  m->e_q = m->fp8_enc ? dalloc<uint8_t>(M * 4 * d) : nullptr;
+  m->e_qs = m->fp8_enc ? dalloc<float>(M) : nullptr;
   m->e_chunks = dalloc<MelChunkDesc>(b);
   m->e_chunk_max = dalloc<int>(b);
   m->enc_max_b = b;
@@ -688,8 +708,30 @@ static const EncPlan& encoder_plan(Model* m, int b) {
     if (epi == EPI_RESID_F32) a.resid = reinterpret_cast<const float*>(out);
     return gemm_plan(a, m->num_sms);
   };
+  // every fp8 GEMM reads its input's codes and row scales from e_q / e_qs, written just before it
+  auto flat8 = [&](int K, const uint8_t* W, const float* ws, int N, const float* bias, void* out, int epi) {
+    Fp8GemmArgs a;
+    a.A = m->e_q;
+    a.a_scale = m->e_qs;
+    a.W = W;
+    a.w_scale = ws;
+    a.rows = M;
+    a.K = K;
+    a.N = N;
+    a.bias = bias;
+    a.out = out;
+    a.epilogue = epi;
+    return gemm_fp8_plan(a, m->num_sms);
+  };
   for (int l = 0; l < Lc; ++l) {
     const EncLayerW& W = m->enc[l];
+    if (m->fp8_enc) {
+      pl.qkv8.push_back(flat8(d, W.q_wqkv, W.s_wqkv, 3 * d, W.bqkv, m->e_qkv, EPI_F16));
+      pl.proj8.push_back(flat8(d, W.q_wo, W.s_wo, d, W.bo, m->e_x, EPI_RESID_F32));
+      pl.ffn1_8.push_back(flat8(d, W.q_w1, W.s_w1, 4 * d, W.b1, m->e_h, EPI_GELU_F16));
+      pl.ffn2_8.push_back(flat8(4 * d, W.q_w2, W.s_w2, d, W.b2, m->e_x, EPI_RESID_F32));
+      continue;
+    }
     pl.qkv.push_back(flat(m->e_xn, d, W.wqkv, 3 * d, W.bqkv, m->e_qkv, EPI_F16));
     pl.proj.push_back(flat(m->e_ao, d, W.wo, d, W.bo, m->e_x, EPI_RESID_F32));
     pl.ffn1.push_back(flat(m->e_xn, d, W.w1, 4 * d, W.b1, m->e_h, EPI_GELU_F16));
@@ -716,6 +758,21 @@ static void encoder_forward(Model* m, int b, __half* dst) {
   run_gemm(m, pl.conv2);
   for (int l = 0; l < m->cfg.n_audio_layer; ++l) {
     const EncLayerW& W = m->enc[l];
+    if (m->fp8_enc) {
+      layernorm_f32_e4m3(m->e_x, W.ln1_g, W.ln1_b, m->e_q, m->e_qs, M, d, s);
+      gemm_fp8_run(pl.qkv8[l], s);
+      if (m->use_ref_attn)
+        attn_ref_run(m->e_qkv, m->e_ao, b, 1500, m->cfg.n_audio_head, s);
+      else
+        attn_run(pl.attn, s);
+      quantize_rows_e4m3(m->e_ao, m->e_q, m->e_qs, M, d, s);
+      gemm_fp8_run(pl.proj8[l], s);
+      layernorm_f32_e4m3(m->e_x, W.ln2_g, W.ln2_b, m->e_q, m->e_qs, M, d, s);
+      gemm_fp8_run(pl.ffn1_8[l], s);
+      quantize_rows_e4m3(m->e_h, m->e_q, m->e_qs, M, 4 * d, s);
+      gemm_fp8_run(pl.ffn2_8[l], s);
+      continue;
+    }
     layernorm_f32_f16(m->e_x, W.ln1_g, W.ln1_b, m->e_xn, M, d, s);
     run_gemm(m, pl.qkv[l]);
     if (m->use_ref_attn)
@@ -1837,7 +1894,8 @@ int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n
     B2W_CHECK(cfg && tensors && out, "null argument");
     require_hopper(device);
     const std::string ct = compute_type ? compute_type : "default";
-    const char* ok[] = {"default", "auto", "float16", "int8_float16", "int8", "float32", "bfloat16", "int8_float32", "int8_bfloat16", "int16"};
+    const char* ok[] = {"default", "auto", "float16", "int8_float16", "int8", "float32", "bfloat16", "int8_float32", "int8_bfloat16", "int16",
+                        "float8_float16"};
     bool known = false;
     for (const char* k : ok) known = known || ct == k;
     if (!known) throw Error("unknown compute_type: " + ct, true);
@@ -1850,7 +1908,10 @@ int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n
     m->num_sms = prop.multiProcessorCount;
     B2W_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
     m->w8 = ct.rfind("int8", 0) == 0;
+    m->fp8_enc = ct == "float8_float16";
     read_env_options(m);
+    if (m->fp8_enc && m->use_ref_gemm)
+      throw Error("compute_type float8_float16 runs the encoder on the e4m3 wgmma GEMM; B2W_GEMM_IMPL=ref has no fp8 path", true);
     TensorTable tt{tensors, n_tensors};
     build_model(m, *cfg, tt);
     *out = h.release();
@@ -2599,6 +2660,78 @@ int b2w_debug_gemm(int32_t device, int32_t impl, b2w_gemm_desc* d) {
       hook_get(d->kcache, ga.kcache, (size_t)d->cache_elems * 2);
       hook_get(d->vcache, ga.vcache, (size_t)d->cache_elems * 2);
     }
+  });
+}
+
+int b2w_debug_gemm_fp8(int32_t device, const uint8_t* a, const float* a_scale, int32_t rows, int32_t K, const uint8_t* w,
+                       const float* w_scale, int32_t N, const float* bias, int32_t epilogue, void* out, int32_t max_ctas) {
+  return guarded([&] {
+    B2W_CHECK(a && a_scale && w && w_scale && out, "null argument");
+    B2W_CHECK(rows >= 1 && K > 0 && K % 64 == 0, "fp8 GEMM K must be a multiple of 64");
+    B2W_CHECK(N > 0 && N % 32 == 0, "fp8 GEMM N must be a multiple of 32");
+    B2W_CHECK(epilogue == EPI_F16 || epilogue == EPI_GELU_F16 || epilogue == EPI_RESID_F32,
+              "fp8 GEMM epilogue is F16, GELU_F16 or RESID_F32");
+    require_hopper(device);
+    DeviceGuard g(device);
+    ScratchBufs hb;
+    const size_t out_bytes = (size_t)rows * N * (epilogue == EPI_RESID_F32 ? 4 : 2);
+    Fp8GemmArgs ga;
+    ga.A = hb.put<uint8_t>(a, (size_t)rows * K);
+    ga.a_scale = hb.put<float>(a_scale, rows);
+    ga.W = hb.put<uint8_t>(w, (size_t)N * K);
+    ga.w_scale = hb.put<float>(w_scale, N);
+    ga.rows = rows;
+    ga.K = K;
+    ga.N = N;
+    ga.bias = bias ? hb.put<float>(bias, N) : nullptr;
+    ga.out = hb.put<uint8_t>(out, out_bytes);
+    ga.epilogue = epilogue;
+    gemm_configure();
+    cudaDeviceProp prop;
+    B2W_CUDA(cudaGetDeviceProperties(&prop, device));
+    Fp8GemmPlan p = gemm_fp8_plan(ga, prop.multiProcessorCount);
+    if (max_ctas > 0) p.grid = std::min(p.grid, (int)max_ctas);
+    gemm_fp8_run(p, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    hook_get(out, ga.out, out_bytes);
+  });
+}
+
+int b2w_debug_quantize_e4m3(int32_t device, const uint16_t* x, int32_t rows, int32_t K, uint8_t* codes, float* scales) {
+  return guarded([&] {
+    B2W_CHECK(x && codes && scales, "null argument");
+    B2W_CHECK(rows >= 1 && K > 0 && K % 8 == 0, "K must be a positive multiple of 8");
+    require_hopper(device);
+    DeviceGuard g(device);
+    ScratchBufs hb;
+    const __half* dx = hb.put<__half>(x, (size_t)rows * K);
+    uint8_t* dq = hb.alloc<uint8_t>((size_t)rows * K);
+    float* ds = hb.alloc<float>(rows);
+    quantize_rows_e4m3(dx, dq, ds, rows, K, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    hook_get(codes, dq, (size_t)rows * K);
+    hook_get(scales, ds, (size_t)rows * 4);
+  });
+}
+
+int b2w_debug_layernorm_e4m3(int32_t device, const float* x, const float* gamma, const float* beta, int32_t rows, int32_t d,
+                             uint8_t* codes, float* scales) {
+  return guarded([&] {
+    B2W_CHECK(x && codes && scales, "null argument");
+    B2W_CHECK((gamma == nullptr) == (beta == nullptr), "LayerNorm gamma and beta come together");
+    B2W_CHECK(rows >= 1 && d > 0 && d % 4 == 0 && d <= 1280, "d must be a multiple of 4 up to 1280");
+    require_hopper(device);
+    DeviceGuard g(device);
+    ScratchBufs hb;
+    const float* dx = hb.put<float>(x, (size_t)rows * d);
+    const float* dg = gamma ? hb.put<float>(gamma, d) : nullptr;
+    const float* db = beta ? hb.put<float>(beta, d) : nullptr;
+    uint8_t* dq = hb.alloc<uint8_t>((size_t)rows * d);
+    float* ds = hb.alloc<float>(rows);
+    layernorm_f32_e4m3(dx, dg, db, dq, ds, rows, d, 0);
+    B2W_CUDA(cudaDeviceSynchronize());
+    hook_get(codes, dq, (size_t)rows * d);
+    hook_get(scales, ds, (size_t)rows * 4);
   });
 }
 

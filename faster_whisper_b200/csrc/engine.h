@@ -77,6 +77,28 @@ void gemm_run(const GemmPlan& p, cudaStream_t stream);
 void gemm_configure();  // per-device kernel attributes; call once per device outside stream capture
 void gemm_ref_run(const GemmArgs& a, cudaStream_t stream);  // plain SIMT reference of the same contract
 
+// e4m3 GEMM of the encoder's linear layers under compute_type float8_float16 (gemm.cu):
+//   out[r][n] = epilogue(a_scale[r] * w_scale[n] * sum_k A[r][k] W[n][k] + bias[n]), A codes [rows][K], W codes [N][K] (fp8.cuh)
+// epilogue EPI_F16 | EPI_GELU_F16 (out fp16 [rows][N]) or EPI_RESID_F32 (out fp32 [rows][N] += ...).  K a multiple of 64.
+struct Fp8GemmArgs {
+  const uint8_t* A = nullptr;
+  const float* a_scale = nullptr;
+  const uint8_t* W = nullptr;
+  const float* w_scale = nullptr;
+  int rows = 0, K = 0, N = 0;
+  const float* bias = nullptr;
+  void* out = nullptr;
+  int epilogue = EPI_F16;
+};
+struct Fp8GemmPlan {
+  Fp8GemmArgs a;
+  CUtensorMap tmA, tmB;
+  int tiles_m = 0, tiles_n = 0, num_kb = 0, grid = 0;
+  double flops() const { return 2.0 * a.rows * (double)a.N * a.K; }
+};
+Fp8GemmPlan gemm_fp8_plan(const Fp8GemmArgs& a, int num_sms);
+void gemm_fp8_run(const Fp8GemmPlan& p, cudaStream_t stream);
+
 // ---- encoder attention on wgmma (attention.cu) ---------------------------------------------------------
 struct AttnPlan {
   const __half* qkv = nullptr;  // [B][T][3*H*64]
@@ -91,6 +113,10 @@ void attn_ref_run(const __half* qkv, __half* out, int B, int T, int H, cudaStrea
 // ---- small encoder kernels (encoder_misc.cu) ---------------------------------------------------------------
 void layernorm_f32_f16(const float* x, const float* gamma, const float* beta, __half* out, int rows, int d, cudaStream_t s);
 void layernorm_f32_f32(const float* x, const float* gamma, const float* beta, float* out, int rows, int d, cudaStream_t s);
+// e4m3 codes [rows][d] + row scales [rows] of the fp32 LayerNorm output, and of fp16 rows [rows][K] (K a multiple of 8)
+void layernorm_f32_e4m3(const float* x, const float* gamma, const float* beta, uint8_t* q, float* scale, int rows, int d,
+                        cudaStream_t s);
+void quantize_rows_e4m3(const __half* x, uint8_t* q, float* scale, int rows, int K, cudaStream_t s);
 void pack_features(const float* feats /*[B][n_mels][3000]*/, __half* out /*[B][3000][cpad]*/, int B, int n_mels, int cpad,
                    cudaStream_t s);
 void convert_f32_f16(const float* in, __half* out, int64_t n, cudaStream_t s);

@@ -301,9 +301,14 @@ static void configure_bn() {
   configure_one<BN, EPI_F32>();
   configure_one<BN, EPI_QKV_CACHE>();
 }
+template <int EPI>
+static void configure_fp8();
 void gemm_configure() {
   configure_bn<32>();
   configure_bn<128>();
+  configure_fp8<EPI_F16>();
+  configure_fp8<EPI_GELU_F16>();
+  configure_fp8<EPI_RESID_F32>();
 }
 
 template <int BN>
@@ -358,6 +363,189 @@ void gemm_run(const GemmPlan& pl, cudaStream_t stream) {
     dispatch_epi<128>(pl, d, stream);
   else
     dispatch_epi<32>(pl, d, stream);
+}
+
+// ---- e4m3 GEMM (compute_type float8_float16) ----------------------------------------------------------------
+// The structure of gemm_tc_kernel with 8-bit operands: 128 x 128 tiles, a K block is one 128-byte swizzle row = 128 codes
+// (16 KB of A + 16 KB of B per stage, the fp16 kernel's stage size; five stages leave room for a 128-column epilogue tile), wgmma m64n128k32 e4m3 x e4m3 -> fp32.  Each K block's
+// four products go into a fresh set of accumulators that is then added to the tile's fp32 sum: the tensor cores' fp8
+// accumulation keeps fewer bits than fp32, so a block's partial sum (128 products) is the most that passes through it.  A K
+// that is a multiple of 64 but not of 128 ends with a half block; TMA fills its upper half with zeros.  The row and column
+// scales multiply the sum in front of the fp16 kernel's epilogues.
+constexpr int kFp8BK = 128;
+constexpr int kFp8Stages = 5;
+constexpr int kFp8ABytes = BM * kFp8BK, kFp8StageBytes = 2 * kFp8ABytes;
+constexpr int kFp8EpiBytes = 2 * 64 * 128 * 4;  // both warpgroups' whole accumulator tiles
+constexpr int kFp8Smem = kFp8Stages * kFp8StageBytes + kFp8EpiBytes + 1024 + 256;
+
+template <int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p,
+                const float* __restrict__ a_scale, const float* __restrict__ w_scale) {
+  constexpr int BN = 128, STAGES = kFp8Stages, STAGE_BYTES = kFp8StageBytes;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* epi = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + kFp8EpiBytes);
+  uint64_t* empty = full + STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  const int total_tiles = p.tiles_m * p.tiles_n;  // tile = m * tiles_n + n
+
+  if (warp == 8) {
+    if (lane == 0) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int n_idx = tile % p.tiles_n, m_idx = tile / p.tiles_n;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_expect_tx(&full[stage], STAGE_BYTES);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          tma_load_2d(sa, &tmA, &full[stage], kb * kFp8BK, m_idx * BM);
+          tma_load_2d(sa + kFp8ABytes, &tmB, &full[stage], kb * kFp8BK, n_idx * BN);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  const int wg = warp >> 2, wq = warp & 3, tig = threadIdx.x & 127;
+  const int g = lane >> 2, t = lane & 3;
+  float* my_epi = epi + wg * 64 * BN;
+  const uint32_t bar_id = 1 + wg;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int n_idx = tile % p.tiles_n, m_idx = tile / p.tiles_n;
+    float acc[BN / 2], part[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = part[i] = 0.f;
+    for (int kb = 0; kb < p.num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+      const uint64_t da = wgmma_desc_sw128(sa + wg * (64 * 128));
+      const uint64_t db = wgmma_desc_sw128(sa + kFp8ABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kFp8BK / 32; ++k) wgmma_ss_e4m3_n128(part, da + 2 * k, db + 2 * k, k);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (tig == 0) mbar_arrive(&empty[stage]);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+
+    // the whole 64 x 128 accumulator tile goes to shared memory at once (one pass keeps no accumulators live next to the
+    // epilogue's operands); 16-byte chunk c of row r sits at c ^ (r % 32)
+    const int row_l = tig & 63, half = tig >> 6;
+    const int row = m_idx * BM + wg * 64 + row_l;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const int col = 8 * i + 2 * t, r = 16 * wq + g;
+      const int c4 = col >> 2, cw = col & 3;
+      *reinterpret_cast<float2*>(my_epi + r * BN + ((c4 ^ (r % 32)) << 2) + cw) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(my_epi + (r + 8) * BN + ((c4 ^ ((r + 8) % 32)) << 2) + cw) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+    for (int c0 = half * 32; c0 < BN; c0 += 64) {
+      const int n0 = n_idx * BN + c0;
+      if (row < p.rows && n0 < p.N) {
+        const float sa_r = __ldg(a_scale + row);
+        const float4* ws4 = reinterpret_cast<const float4*>(w_scale + n0);
+        float v[32];
+        const float4* src = reinterpret_cast<const float4*>(my_epi + row_l * BN);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 f = src[(c0 / 4 + i) ^ (row_l % 32)];
+          const float4 ws = __ldg(ws4 + i);
+          v[4 * i] = f.x * (sa_r * ws.x);
+          v[4 * i + 1] = f.y * (sa_r * ws.y);
+          v[4 * i + 2] = f.z * (sa_r * ws.z);
+          v[4 * i + 3] = f.w * (sa_r * ws.w);
+        }
+        epilogue_store<EPI>(p, 0, row, n0, v);
+      }
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+  }
+}
+
+Fp8GemmPlan gemm_fp8_plan(const Fp8GemmArgs& a, int num_sms) {
+  B2W_CHECK(a.K % 64 == 0 && a.K > 0, "fp8 GEMM K must be a multiple of 64");
+  B2W_CHECK(a.N % 32 == 0 && a.N > 0 && a.rows > 0, "fp8 GEMM N must be a multiple of 32");
+  B2W_CHECK(a.epilogue == EPI_F16 || a.epilogue == EPI_GELU_F16 || a.epilogue == EPI_RESID_F32,
+            "fp8 GEMM epilogue is F16, GELU_F16 or RESID_F32");
+  Fp8GemmPlan p;
+  p.a = a;
+  p.tiles_m = ceil_div(a.rows, BM);
+  p.tiles_n = ceil_div(a.N, 128);
+  p.num_kb = ceil_div(a.K, kFp8BK);
+  const long long total = (long long)p.tiles_m * p.tiles_n;
+  p.grid = (int)(total < num_sms ? total : num_sms);
+  {
+    uint64_t dims[2] = {(uint64_t)a.K, (uint64_t)a.rows};
+    uint64_t strides[1] = {(uint64_t)a.K};
+    uint32_t box[2] = {kFp8BK, BM};
+    p.tmA = make_tmap_u8(a.A, 2, dims, strides, box);
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)a.K, (uint64_t)a.N};
+    uint64_t strides[1] = {(uint64_t)a.K};
+    uint32_t box[2] = {kFp8BK, 128};
+    p.tmB = make_tmap_u8(a.W, 2, dims, strides, box);
+  }
+  return p;
+}
+
+template <int EPI>
+static void configure_fp8() {
+  B2W_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFp8Smem));
+}
+
+template <int EPI>
+static void launch_fp8(const Fp8GemmPlan& pl, const GemmDev& d, cudaStream_t stream) {
+  gemm_fp8_kernel<EPI><<<pl.grid, kGemmThreads, kFp8Smem, stream>>>(pl.tmA, pl.tmB, d, pl.a.a_scale, pl.a.w_scale);
+  B2W_LAUNCHED();
+}
+
+void gemm_fp8_run(const Fp8GemmPlan& pl, cudaStream_t stream) {
+  GemmDev d{};
+  d.batch = 1;
+  d.tiles_m = pl.tiles_m;
+  d.tiles_n = pl.tiles_n;
+  d.num_kb = pl.num_kb;
+  d.rows = pl.a.rows;
+  d.N = pl.a.N;
+  d.bias = pl.a.bias;
+  d.out = pl.a.out;
+  d.out_ld = pl.a.N;
+  d.resid = reinterpret_cast<const float*>(pl.a.out);
+  switch (pl.a.epilogue) {
+    case EPI_F16: launch_fp8<EPI_F16>(pl, d, stream); break;
+    case EPI_GELU_F16: launch_fp8<EPI_GELU_F16>(pl, d, stream); break;
+    case EPI_RESID_F32: launch_fp8<EPI_RESID_F32>(pl, d, stream); break;
+    default: throw Error("unknown fp8 GEMM epilogue");
+  }
 }
 
 // ---- plain SIMT reference with the same contract (debug / bisecting; never the timed path) -----------------
@@ -425,8 +613,8 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                          const uint32_t* box) {
+static CUtensorMap make_tmap(CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                             const uint64_t* strides_bytes, const uint32_t* box) {
   static PFN_encodeTiled fn = nullptr;
   if (!fn) {
     void* sym = nullptr;
@@ -445,7 +633,7 @@ CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, cons
     estrides[i] = 1;
   }
   for (int i = 0; i + 1 < rank; ++i) gstrides[i] = strides_bytes[i];
-  CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdims, gstrides, bdims,
+  CUresult r = fn(&m, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdims, gstrides, bdims,
                   estrides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -457,6 +645,14 @@ CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, cons
     throw Error(buf);
   }
   return m;
+}
+
+CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                          const uint32_t* box) {
+  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, rank, dims, strides_bytes, box);
+}
+CUtensorMap make_tmap_u8(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box);
 }
 
 }  // namespace b2w

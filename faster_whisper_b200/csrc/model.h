@@ -18,8 +18,11 @@ namespace b2w {
 
 struct EncLayerW {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b;
-  __half *wqkv, *wo, *w1, *w2;
+  __half *wqkv, *wo, *w1, *w2;  // NULL under compute_type float8_float16
   float *bqkv, *bo, *b1, *b2;
+  // compute_type float8_float16: e4m3 codes and per-output-channel scales of the four linear layers (fp8.cuh)
+  uint8_t *q_wqkv, *q_wo, *q_w1, *q_w2;
+  float *s_wqkv, *s_wo, *s_w1, *s_w2;
 };
 struct DecLayerW {  // every LayerNorm affine is folded into the projection that consumes it (fold_ln)
   __half *wqkv, *wo, *wq_x, *wo_x, *w1, *w2;
@@ -30,6 +33,7 @@ struct EncPlan {  // everything bound to the encoder workspace for one sub-batch
   int b = 0;
   GemmPlan conv1, conv2;
   std::vector<GemmPlan> qkv, proj, ffn1, ffn2;
+  std::vector<Fp8GemmPlan> qkv8, proj8, ffn1_8, ffn2_8;  // compute_type float8_float16
   AttnPlan attn;
 };
 
@@ -98,6 +102,8 @@ struct Model {
   __half* e_qkv = nullptr;    // [b*1500][3d]
   __half* e_ao = nullptr;     // [b*1500][d]
   __half* e_h = nullptr;      // [b*1500][4d]
+  uint8_t* e_q = nullptr;     // float8_float16: e4m3 codes of the next linear layer's input, [b*1500][up to 4d]
+  float* e_qs = nullptr;      // their row scales [b*1500]
   float* e_pcm = nullptr;     // audio staging
   size_t e_pcm_cap = 0;
   MelChunkDesc* e_chunks = nullptr;
@@ -132,6 +138,8 @@ struct Model {
   // compute_type int8*: the decoder's linear layers (and the output embedding) are quantised per output channel; the persistent step
   // kernels stream them as int8 (w8), every other path uses the de-quantised fp16 values.
   bool w8 = false;
+  // compute_type float8_float16: the encoder's QKV, out-projection, FFN1 and FFN2 run as e4m3 GEMMs (gemm_fp8_kernel)
+  bool fp8_enc = false;
   // many-row persistent step kernel (bstep.cu): decoder weights as 16 KB wgmma atoms + per-row sums for the deferred LayerNorm
   bool bstep_packed = false;
   BLayer* d_blayers = nullptr;

@@ -145,7 +145,7 @@ ABI_SYMBOLS = (
     "b2w_model_info", "b2w_model_sync", "b2w_logmel", "b2w_logmel_frames", "b2w_encode", "b2w_encode_audio",
     "b2w_encoded_shape", "b2w_encoded_to_host", "b2w_encoded_free", "b2w_encoded_split", "b2w_memory_get", "b2w_generate",
     "b2w_gen_opts_default", "b2w_detect_language", "b2w_align", "b2w_align_batch", "b2w_align_items", "b2w_model_set_alignment_heads", "b2w_timing_enable", "b2w_timing_reset", "b2w_timing_get", "b2w_span_begin", "b2w_span_end",
-    "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
+    "b2w_counters_get", "b2w_debug_gemm", "b2w_debug_gemm_fp8", "b2w_debug_quantize_e4m3", "b2w_debug_layernorm_e4m3", "b2w_debug_attention", "b2w_debug_gemv", "b2w_debug_logits", "b2w_debug_fetch",
     "b2w_debug_step_logits", "b2w_debug_self_attn", "b2w_debug_cross_attn", "b2w_debug_search", "b2w_debug_align_cost", "b2w_debug_dtw", "b2w_vad_create", "b2w_vad_destroy", "b2w_vad_probs", "b2w_vad_probs_multi", "b2w_vad_set_block", "b2w_vad_timing",
     "b2w_session_create", "b2w_session_push", "b2w_session_run", "b2w_session_pending", "b2w_session_counters", "b2w_session_destroy",
     "b2w_session_debug_record", "b2w_session_debug_logits",
@@ -208,6 +208,11 @@ def load_library():
         lib.b2w_span_end.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         lib.b2w_counters_get.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
         lib.b2w_debug_gemm.argtypes = [C.c_int32, C.c_int32, C.POINTER(_GemmDesc)]
+        lib.b2w_debug_gemm_fp8.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                           C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]
+        lib.b2w_debug_quantize_e4m3.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        lib.b2w_debug_layernorm_e4m3.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                                 C.c_void_p]
         lib.b2w_debug_attention.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         lib.b2w_debug_gemv.argtypes = [C.c_int32, C.c_int32, C.POINTER(_GemvDesc)]
         lib.b2w_debug_logits.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
@@ -396,8 +401,9 @@ class _Replica:
             pass
 
 
+# float8_float16: the encoder's linear layers as e4m3 tensor-core GEMMs, everything else as float16 (include/b200whisper.h)
 _COMPUTE_TYPES = ("default", "auto", "int8", "int8_float32", "int8_float16", "int8_bfloat16", "int16", "float16",
-                  "bfloat16", "float32")
+                  "bfloat16", "float32", "float8_float16")
 
 
 class Whisper:
@@ -1043,6 +1049,44 @@ def debug_gemm(a: np.ndarray, w: np.ndarray, bias: Optional[np.ndarray], impl: i
     out = np.zeros((a16.shape[0], w16.shape[0]), np.float16 if gelu else np.float32)
     debug_gemm_desc(a16, w16, out, epilogue=EPI_GELU_F16 if gelu else EPI_F32, rows=a16.shape[0], bias=bias, impl=impl, device=device)
     return out.astype(np.float32)
+
+
+def debug_gemm_fp8(a: np.ndarray, a_scale: np.ndarray, w: np.ndarray, w_scale: np.ndarray, out: np.ndarray, *, epilogue: int,
+                   bias: Optional[np.ndarray] = None, max_ctas: int = 0, device: int = 0) -> None:
+    """The encoder's e4m3 GEMM (b2w_debug_gemm_fp8; tests only): a uint8 codes [rows, K], w uint8 codes [N, K], float32 row /
+    channel scales; out (float16 [rows, N] for EPI_F16 / EPI_GELU_F16, float32 for EPI_RESID_F32) is updated in place."""
+    lib = load_library()
+    a, w = _buf(a, np.uint8, "a"), _buf(w, np.uint8, "w")
+    a_scale, w_scale = _buf(a_scale, np.float32, "a_scale"), _buf(w_scale, np.float32, "w_scale")
+    out = _buf(out, np.float16 if epilogue in EPI_F16_OUT else np.float32, "out")
+    bias = None if bias is None else np.ascontiguousarray(bias, np.float32)
+    (rows, K), N = a.shape, w.shape[0]
+    if w.shape[1] != K or a_scale.shape != (rows,) or w_scale.shape != (N,) or out.shape != (rows, N) or (bias is not None and bias.shape != (N,)):
+        raise ValueError("shapes: a [rows, K], w [N, K], a_scale [rows], w_scale [N], out [rows, N], bias [N]")
+    _check(lib.b2w_debug_gemm_fp8(device, _ptr(a), _ptr(a_scale), rows, K, _ptr(w), _ptr(w_scale), N, _ptr(bias), epilogue, _ptr(out),
+                                  max_ctas))
+
+
+def debug_quantize_e4m3(x: np.ndarray, device: int = 0) -> Tuple[np.ndarray, np.ndarray]:
+    """e4m3 codes (uint8 [rows, K]) and row scales (float32 [rows]) of float16 rows x [rows, K] (tests only)."""
+    lib = load_library()
+    x = _buf(x, np.float16, "x")
+    rows, K = x.shape
+    codes, scales = np.zeros((rows, K), np.uint8), np.zeros(rows, np.float32)
+    _check(lib.b2w_debug_quantize_e4m3(device, _ptr(x), rows, K, _ptr(codes), _ptr(scales)))
+    return codes, scales
+
+
+def debug_layernorm_e4m3(x: np.ndarray, gamma: Optional[np.ndarray], beta: Optional[np.ndarray], device: int = 0) -> Tuple[np.ndarray, np.ndarray]:
+    """e4m3 codes and row scales of the float32 LayerNorm(x) * gamma + beta of float32 rows x [rows, d] (tests only)."""
+    lib = load_library()
+    x = _buf(x, np.float32, "x")
+    gamma = None if gamma is None else np.ascontiguousarray(gamma, np.float32)
+    beta = None if beta is None else np.ascontiguousarray(beta, np.float32)
+    rows, d = x.shape
+    codes, scales = np.zeros((rows, d), np.uint8), np.zeros(rows, np.float32)
+    _check(lib.b2w_debug_layernorm_e4m3(device, _ptr(x), _ptr(gamma), _ptr(beta), rows, d, _ptr(codes), _ptr(scales)))
+    return codes, scales
 
 
 def debug_attention(qkv: np.ndarray, heads: int, impl: int = 0, device: int = 0):

@@ -80,7 +80,10 @@ int b2w_device_count(int* count);
 /* ctranslate2.models.Whisper(model_path, device, device_index, compute_type, ...) (transcribe.py:689-698).
  * compute_type: "float16" | "default" | "auto" -> fp16 weights; "int8" | "int8_float16" | ... -> the decoder's linear layers and the
  * output embedding are quantised per output channel (symmetric, scale = max|w|/127) at load; the single-stream decode kernel
- * streams them as int8 and applies the scale to the fp32 sums, all other paths multiply with the de-quantised fp16 values. */
+ * streams them as int8 and applies the scale to the fp32 sums, all other paths multiply with the de-quantised fp16 values.
+ * "float8_float16" -> the encoder's four linear layers per block (QKV, out-projection, FFN1, FFN2) run as e4m3 tensor-core GEMMs:
+ * weights quantised per output channel at load, their inputs per token row (b2w_debug_quantize_e4m3's rule); everything else,
+ * the decoder included, is as "float16". */
 int b2w_model_create(const b2w_config* cfg, const b2w_tensor* tensors, int32_t n_tensors, int32_t device,
                      const char* compute_type, b2w_model** out);
 void b2w_model_destroy(b2w_model* m);
@@ -282,6 +285,18 @@ typedef struct b2w_gemm_desc {
 /* Run one described GEMM through the wgmma kernel (impl=0) or the plain SIMT reference of the same contract (impl=1).  Every
  * argument (shapes, strides, buffer extents, row table) is checked before anything runs on the device. */
 int b2w_debug_gemm(int32_t device, int32_t impl, b2w_gemm_desc* desc);
+/* compute_type "float8_float16": the encoder's e4m3 GEMM on given codes (e4m3 bytes) and scales, a [rows][K] and w [N][K]
+ * (K a multiple of 64, N of 32): out[r][n] = epilogue(a_scale[r] * w_scale[n] * sum_k a[r][k] w[n][k] + bias[n]) for epilogue
+ * B2W_EPI_F16 or B2W_EPI_GELU_F16 (out fp16 [rows][N]) or B2W_EPI_RESID_F32 (out float32 [rows][N], added to in place).  bias
+ * may be NULL; max_ctas as in b2w_gemm_desc.  Arguments are checked before any device work. */
+int b2w_debug_gemm_fp8(int32_t device, const uint8_t* a, const float* a_scale, int32_t rows, int32_t K, const uint8_t* w,
+                       const float* w_scale, int32_t N, const float* bias, int32_t epilogue, void* out, int32_t max_ctas);
+/* The encoder's e4m3 row quantisation (per row: scale = amax / 448, 1 when amax is 0; code = e4m3(x / scale), round to nearest
+ * even, saturating): of fp16 rows x [rows][K] (K a multiple of 8), and of the float32 LayerNorm output of x [rows][d] (gamma and
+ * beta both NULL for no affine).  codes [rows][K|d], scales [rows]. */
+int b2w_debug_quantize_e4m3(int32_t device, const uint16_t* x, int32_t rows, int32_t K, uint8_t* codes, float* scales);
+int b2w_debug_layernorm_e4m3(int32_t device, const float* x, const float* gamma, const float* beta, int32_t rows, int32_t d,
+                             uint8_t* codes, float* scales);
 /* softmax(QK^T/8)V for [B,T,H*64] fp16-rounded inputs through the wgmma (0) or reference (1) kernel. */
 int b2w_debug_attention(int32_t device, int32_t impl, const float* qkv, int32_t B, int32_t T, int32_t H,
                         float* out);
